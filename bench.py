@@ -1,16 +1,19 @@
 #!/usr/bin/env python3
 """bench.py -- the hot-path benchmark (driver contract).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workload c2|c3|c4|c5]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workload c2|c3|c4|c5] [--dump-outputs DIR]
 
-One "step" = one pass of the workload's op list over one batch of synthetic frames.  Default workload = BASELINE.json
-configs[1] ("c2"): the filter2D / sepFilter2D / GaussianBlur sweep 3x3..31x31 on 3840x2160 CV_8UC1 and CV_32FC1.
+One "step" = one pass of the workload's op list over one batch of synthetic frames.  Default workload "c2": the
+filter2D / sepFilter2D / GaussianBlur sweep 3x3..31x31 on 3840x2160 CV_8UC1 and CV_32FC1.
 Prints ONE JSON line (rank 0):  metric = Mpix/s (destination pixels of every op, whole job), `value` = device-resident,
 `e2e` = same ops through the host C ABI (pinned host buffers, H2D + D2H inside the timed region), `roofline` for the
 kernel with the largest share of the step, `per_op` for every op, `cpu_baseline` = the reference's own CPU path
 (oracle/_ref, or the C port when that is absent) on a bounded sample, `clocks` sampled during the timed region.
 Multi-GPU (torchrun): frames shard across ranks (weak scaling); the only collective is an NCCL broadcast of the filter
 taps / template per step.
+--dump-outputs DIR: after the timed steps, rank 0 writes what every op of the --workload pass returned in the last step as DIR/<op>.npy
+(float32, float64 for float64 results; a fixed, seeded sample of elements where an output is larger than its share of 64 MB).  Inputs
+are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -35,12 +38,12 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3 3.35 TB/s), not measured"
 
 
 # ------------------------------------------------------------------------------------------------------------------
 # workload definitions: list of ops; each op = dict(name, make(ctx)->callable, px (dst pixels per frame), bytes (algorithmic
-# bytes per frame, SURVEY 8d), frames)
+# bytes per frame: source read once, destination written once), frames)
 # ------------------------------------------------------------------------------------------------------------------
 def gauss_taps(k):
     import opencv_b200 as cvb
@@ -255,7 +258,33 @@ def make_extra(ops, rng, need_device):
     return extra
 
 
-def measure_device(workload, steps, W, use_graph, rank, world, local, rng, sample_clocks=True):
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(ops, out_dir):
+    """every op's result of the last step -> out_dir/<op>.npy (<op>.<i>.npy for the parts of a tuple result).  An output larger than its
+    share of DUMP_BYTES is sampled at fixed positions: a seeded draw that depends only on the op name and the output size."""
+    import zlib
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    outs = []
+    for op in ops:
+        r = op["_dst"] if op["_dst"] is not None else op.get("_out")
+        parts = [r] if not isinstance(r, (tuple, list)) else list(r)
+        parts = [torch.as_tensor(p) if isinstance(p, np.ndarray) else p for p in parts if isinstance(p, (torch.Tensor, np.ndarray))]
+        for i, t in enumerate(parts):
+            outs.append((op["name"] if len(parts) == 1 else "%s.%d" % (op["name"], i), t))
+    share = DUMP_BYTES // 8 // max(1, len(outs))         # elements per output, sized for float64
+    for name, t in outs:
+        flat = t.reshape(-1)
+        if flat.numel() > share:
+            idx = np.sort(np.random.default_rng(zlib.crc32(name.encode())).integers(0, flat.numel(), share))
+            flat = flat[torch.from_numpy(idx).to(flat.device)]
+        a = flat.cpu().numpy()
+        np.save(os.path.join(out_dir, name + ".npy"), a.astype(np.float64 if a.dtype == np.float64 else np.float32))
+
+
+def measure_device(workload, steps, W, use_graph, rank, world, local, rng, sample_clocks=True, dump_dir=None):
     """device-resident pass of one workload: returns (result dict, ops, extra, bufs).  value = Mpix/s over `steps` steps (CUDA events, max over ranks)"""
     import torch
     import torch.distributed as dist
@@ -267,8 +296,8 @@ def measure_device(workload, steps, W, use_graph, rank, world, local, rng, sampl
     # device-resident inputs / outputs: one buffer per distinct spec (every op's in+out working set > L2)
     bufs = {}
 
-    def buf(spec, fill):
-        key = (spec[0], np.dtype(spec[1]).str, fill)
+    def buf(spec, fill, owner=None):
+        key = (spec[0], np.dtype(spec[1]).str, fill) + ((owner,) if owner else ())
         if key not in bufs:
             shp, dt = spec
             tdt = torch.uint8 if np.dtype(dt) == np.uint8 else torch.float32
@@ -282,7 +311,8 @@ def measure_device(workload, steps, W, use_graph, rank, world, local, rng, sampl
 
     for op in ops:
         op["_src"] = buf(op["src"], True)
-        op["_dst"] = buf(op["dst"], False) if op["dst"] is not None else None
+        # with --dump-outputs every op writes its own buffer, so that the last step leaves every result; otherwise ops share them
+        op["_dst"] = buf(op["dst"], False, op["name"] if dump_dir else None) if op["dst"] is not None else None
     if workload == "c4":
         extra["templ"] = ops[0]["_src"][0, 700:764, 1000:1064, 0].contiguous()
 
@@ -330,7 +360,9 @@ def measure_device(workload, steps, W, use_graph, rank, world, local, rng, sampl
         for i, op in enumerate(ops):
             if record:
                 ev[i][0].record()
-            run_op(cvb, op, op["_src"], op["_dst"], extra)
+            ret = run_op(cvb, op, op["_src"], op["_dst"], extra)
+            if op["_dst"] is None:
+                op["_out"] = ret         # results the op allocates (a captured graph rewrites the same memory on every replay)
             if record:
                 ev[i][1].record()
 
@@ -394,6 +426,8 @@ def measure_device(workload, steps, W, use_graph, rank, world, local, rng, sampl
     sampler.stop_flag = True
     if sample_clocks:
         sampler.join(timeout=2)
+    if dump_dir and rank == 0:
+        dump_outputs(ops, dump_dir)
     # per-op times: eager steps with an event pair around every op (outside the timed region; the first pass re-warms the
     # stream-ordered allocator after the graph replays)
     shared_operands()
@@ -418,27 +452,21 @@ def measure_device(workload, steps, W, use_graph, rank, world, local, rng, sampl
         per_op[op["name"]] = {"ms": round(float(ms), 4), "mpix_s": round(op["px"] * op["frames"] / (ms * 1e-3) / 1e6, 1), "gbs": round(gbs, 1), "frac_hbm": round(gbs / peak, 4)}
     dom = int(np.argmax(per_op_ms))
     dgbs = ops[dom]["abytes"] * ops[dom]["frames"] / (per_op_ms[dom] * 1e-3) / 1e9
-    # dram bytes per launch of the op's main kernel from `ncu --set full` (profiles/ncu_traffic.json, written from the committed captures)
-    traffic = None
-    try:
-        with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "ncu_traffic.json")) as fh:
-            traffic = json.load(fh).get(ops[dom]["name"])
-    except (OSError, ValueError):
-        traffic = None
-    roofline = {"kernel": ops[dom]["name"], "bound": "hbm", "achieved": round(dgbs, 1), "peak": peak, "unit": "GB/s", "frac": round(dgbs / peak, 4), "traffic": traffic,
+    roofline = {"kernel": ops[dom]["name"], "bound": "hbm", "achieved": round(dgbs, 1), "peak": peak, "unit": "GB/s", "frac": round(dgbs / peak, 4),
                 "peak_source": peak_src, "share_of_step": round(float(per_op_ms[dom] / per_op_ms.sum()), 3),
-                "note": "dominant = largest share of step time; per_op lists achieved GB/s and HBM fraction of every op (algorithmic bytes, SURVEY 8d)"}
+                "note": "dominant = largest share of step time; per_op lists achieved GB/s and HBM fraction of every op (algorithmic bytes: source read once, destination written once)"}
     if ops[dom]["kind"] == "f2d":
         k = ops[dom]["k"]
         is_f32 = np.dtype(ops[dom]["src"][1]) == np.float32
         tfl = 2.0 * k * k * ops[dom]["px"] * ops[dom]["frames"] / (per_op_ms[dom] * 1e-3) / 1e12
         if k * k >= 130 and k >= 13:
-            # from the reference's DFT switch on (130 taps) filter2D is a dense contraction on tcgen05: the tensor pipe bounds it, not HBM.
+            # from the reference's DFT switch on (130 taps) filter2D is a dense contraction on the tensor cores (wgmma): the tensor pipe bounds it, not HBM.
             # achieved = ALGORITHMIC flops (2 k^2 per pixel).  The MMAs issue more: the Toeplitz form pads every kernel row to K = k + 31 -> 48 / 64
             # columns, and float images run 3 x BF16 as two MMAs per K step (N = 64 + N = 32): 96 K MACs per 32 pixels per kernel row and K step.
-            tpeak = 1681.6
+            tpeak, tpeak_src = 989.4, "H100 SXM data sheet (dense BF16), not measured"
             try:
                 tpeak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["bf16_tflops"])
+                tpeak_src = "measured (MEASURED_PEAKS.json bf16_tflops, burst)"
             except (OSError, ValueError, KeyError):
                 pass
             K = 16 * ((k + 31 + 15) // 16) if is_f32 else 64
@@ -446,18 +474,21 @@ def measure_device(workload, steps, W, use_graph, rank, world, local, rng, sampl
             itfl = issued_per_px * ops[dom]["px"] * ops[dom]["frames"] / (per_op_ms[dom] * 1e-3) / 1e12
             ipeak = tpeak if is_f32 else 2 * tpeak
             roofline.update({"bound": "tensor", "achieved": round(tfl, 1), "peak": tpeak, "unit": "TFLOP/s", "frac": round(tfl / tpeak, 4),
-                             "peak_source": "measured (MEASURED_PEAKS.json bf16_tflops, burst)",
+                             "peak_source": tpeak_src,
                              "hbm": {"achieved": round(dgbs, 1), "peak": peak, "unit": "GB/s", "frac": round(dgbs / peak, 4)},
                              "issued": {"achieved": round(itfl, 1), "peak": ipeak, "unit": "TFLOP/s" if is_f32 else "TOP/s", "frac": round(itfl / ipeak, 3),
                                         "note": "MMA volume actually issued (Toeplitz zeros and the %s included) against the %s peak; the op time includes the border-extension / split kernel"
-                                                % ("3 x BF16 split" if is_f32 else "three base-256 tap digits", "measured bf16" if is_f32 else "int8 = 2 x measured bf16")},
-                             "note": "dominant = largest share of step time; a >= 130-tap filter2D is a tcgen05 contraction (kind::%s): tensor bound, achieved = algorithmic flops 2 k^2 per pixel; "
-                                     "ncu: tensor pipe active ~50 %%, shared-memory operand wavefronts ~90 %% of peak (profiles/)" % ("f16, BF16 operands" if is_f32 else "i8")})
+                                                % ("3 x BF16 split" if is_f32 else "three base-256 tap digits", "bf16" if is_f32 else "int8 = 2 x bf16")},
+                             "note": "dominant = largest share of step time; a >= 130-tap filter2D is a wgmma contraction (%s): tensor bound, achieved = algorithmic flops 2 k^2 per pixel"
+                                     % ("BF16 operands, FP32 accumulators" if is_f32 else "u8 x s8 -> s32")})
         else:
             # below that a k x k direct sum is k*k FMA per pixel: the FP32 pipe, not HBM, bounds it -- report that too
-            fp32_peak = 148 * 128 * 2 * 1.965e9 / 1e12
+            n_sm = torch.cuda.get_device_properties(dev).multi_processor_count
+            mhz = (sampler.summary()["sm_max_mhz"] if sample_clocks else None) or 1980.0
+            fp32_peak = n_sm * 128 * 2 * mhz * 1e6 / 1e12
             roofline["fp32"] = {"achieved": round(tfl, 1), "peak": round(fp32_peak, 1), "unit": "TFLOP/s", "frac": round(tfl / fp32_peak, 3),
-                                "note": "148 SM x 128 FMA lanes x 2 x 1.965 GHz; this op is FMA-issue bound (k*k MAC per pixel), its HBM fraction is not the limiter"}
+                                "note": "%d SM x 128 FMA lanes x 2 x %.0f MHz (maximum SM clock); this op is FMA-issue bound (k*k MAC per pixel), its HBM fraction is not the limiter"
+                                        % (n_sm, mhz)}
 
     res = {"value": value, "total_ms": total_ms, "ms_per_step": total_ms / steps, "per_op": per_op, "roofline": roofline, "launches": int(launches),
            "launches_per_step": int(launches_per_step), "graph_note": graph_note, "host_enqueue_ms": host_enqueue_ms, "clocks": sampler.summary() if sample_clocks else None, "desc": desc}
@@ -492,9 +523,9 @@ def measure_e2e(workload, ops, extra, bufs, steps, rank, world, local):
     hextra = dict(extra)
     if "templ" in extra:
         hextra["templ"] = extra["templ"].cpu().numpy()
-    hsteps = max(1, min(steps, 3))
+    hsteps = steps
     if workload == "c5":
-        # C5 end to end: host frames in, waves of pyramids + DoG kept on the device for the consumer of the wave (SURVEY 7.2: 1.9 GB per
+        # C5 end to end: host frames in, waves of pyramids + DoG kept on the device for the consumer of the wave (1.9 GB per
         # frame cannot come back over PCIe), Harris responses downloaded.  32 frames per rank per step; 1024 frames = 4 steps on 8 ranks.
         nf = 32
         sspec = ((nf, H4K, W4K, 1), np.uint8)
@@ -576,6 +607,7 @@ def main():
     ap.add_argument("--no-graph", action="store_true", help="issue every launch from the host each step instead of replaying a captured CUDA graph")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the short C3/C4/C5 passes that ride along with the default (C2) workload")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the outputs of the last timed step of the --workload pass (not of the c3/c4/c5 passes that ride along with c2) as DIR/<op>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0")); world = int(os.environ.get("WORLD_SIZE", "1")); local = int(os.environ.get("LOCAL_RANK", "0"))
     rng = np.random.default_rng(0x5EED0000 + 2 + rank)
@@ -619,7 +651,7 @@ def main():
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
     dev = torch.device("cuda", local)
-    res, ops, extra, bufs = measure_device(args.workload, args.steps, W, not args.no_graph, rank, world, local, rng)
+    res, ops, extra, bufs = measure_device(args.workload, args.steps, W, not args.no_graph, rank, world, local, rng, dump_dir=args.dump_outputs)
     value, total_ms, per_op, roofline, launches = res["value"], res["total_ms"], res["per_op"], res["roofline"], res["launches"]
     graph_note, host_enqueue_ms, desc = res["graph_note"], res["host_enqueue_ms"], res["desc"]
 
@@ -639,7 +671,7 @@ def main():
         except Exception as exc:                        # noqa: BLE001
             e2e["per_call_hal"] = {"error": repr(exc)[:200]}
 
-    # ---------------- the other BASELINE configs (C3, C4, C5) measured in the same run: short device-resident passes with per-op tables --------
+    # ---------------- the other workloads (C3, C4, C5) measured in the same run: short device-resident passes with per-op tables --------
     extra_workloads = None
     if args.workload == "c2" and not args.no_extra:
         for op in ops:                                  # release the main workload's device and pinned buffers first
@@ -650,11 +682,11 @@ def main():
         extra_workloads = {}
         for w in ("c3", "c4", "c5"):
             try:
-                r, o2, x2, b2 = measure_device(w, max(1, min(args.steps, 3)), 3, not args.no_graph, rank, world, local, np.random.default_rng(0x5EED0000 + ord(w[1]) + rank), sample_clocks=False)
+                r, o2, x2, b2 = measure_device(w, args.steps, 3, not args.no_graph, rank, world, local, np.random.default_rng(0x5EED0000 + ord(w[1]) + rank), sample_clocks=False)
                 extra_workloads[w] = {"workload": r["desc"], "value": r["value"], "unit": "Mpix/s", "ms_per_step": r["ms_per_step"], "launch": r["graph_note"],
                                       "gpu_launches_per_step": r["launches_per_step"], "per_op": r["per_op"]}
                 if not args.no_e2e:
-                    extra_workloads[w]["e2e"] = measure_e2e(w, o2, x2, b2, 2, rank, world, local)
+                    extra_workloads[w]["e2e"] = measure_e2e(w, o2, x2, b2, args.steps, rank, world, local)
                 for op in o2:
                     for k in ("_src", "_dst", "_hsrc", "_hdst"):
                         op.pop(k, None)
@@ -684,7 +716,7 @@ def main():
     if rank == 0:
         out = {"metric": "Mpix/s", "value": value, "unit": "Mpix/s", "n_gpus": world, "steps": args.steps, "warmup": W,
                "ms_per_step": total_ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u8/f32",
-               "data": "synthetic", "config": {"workload": desc, "l2": "every op streams a batch whose input+output exceed the 126 MB L2",
+               "data": "synthetic", "config": {"workload": desc, "l2": "every op streams a batch whose input+output exceed the 50 MB L2",
                                                 "parallelism": "frames sharded across %d rank(s); NCCL broadcast of taps/kernels per step" % world,
                                                 "launch": graph_note, "host_enqueue_ms_per_step": round(host_enqueue_ms, 3)},
                "gpu_launches": int(launches), "clocks": res["clocks"], "roofline": roofline, "per_op": per_op}

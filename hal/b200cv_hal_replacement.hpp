@@ -3,7 +3,7 @@
 // Registered through OpenCV's own mechanism (CMakeLists.txt:927-1040, samples/hal/README.md):
 //     cmake -DOpenCV_HAL_DIR=<repo>/hal  ...        (hal/b200cv_halConfig.cmake names this header + libb200cv.so)
 // modules/imgproc/src/hal_replacement.hpp then includes it via custom_hal.hpp (:1339) and every `cv_hal_X` below stops being
-// the NOT_IMPLEMENTED stub (`hal_ni_X`) and becomes the B200 path.  Semantics of the return value are the seam's
+// the NOT_IMPLEMENTED stub (`hal_ni_X`) and becomes the GPU path.  Semantics of the return value are the seam's
 // (hal_replacement.hpp:1342-1357): 0 = done, 1 = not implemented -> OpenCV runs its own code, anything else -> cv::Error.
 #ifndef B200CV_HAL_REPLACEMENT_HPP
 #define B200CV_HAL_REPLACEMENT_HPP

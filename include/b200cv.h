@@ -1,5 +1,5 @@
 /*
- * b200cv.h -- C ABI of the B200-native dense-imgproc hot path (OpenCV drop-in boundary).
+ * b200cv.h -- C ABI of the H100-native dense-imgproc hot path (OpenCV drop-in boundary).
  *
  * Plain C: pointers, sizes, ints, doubles.  No C++ / torch / OpenCV types cross this line.
  * Everything above it (the cv::-signature C++ mirror in opencv_b200/host/, the cv_hal_*
@@ -179,14 +179,14 @@ B200CV_API int b200cv_warp_affine(const b200cvMat* src, const b200cvMat* dst, co
 /* replaces cv::warpPerspective (imgproc.hpp:2482; imgwarp.cpp:3370-3466). M: 3x3 doubles. */
 B200CV_API int b200cv_warp_perspective(const b200cvMat* src, const b200cvMat* dst, const double* M, int flags,
                                        int border, const double* border_value, void* stream);
-/* replaces cv::remap (imgproc.hpp:2531; imgwarp.cpp:1762-1900, RemapInvoker :1096-1330) -- SURVEY 8(f) "next": the caller of the
+/* replaces cv::remap (imgproc.hpp:2531; imgwarp.cpp:1762-1900, RemapInvoker :1096-1330) -- the caller of the
  * sampling code the warps already use.  dst has the size of the maps and the type of src.  Maps (one set for the whole batch):
  *   map1 CV_32FC1 + map2 CV_32FC1 (x and y planes), map1 CV_32FC2 (map2 NULL), or the fixed-point pair of cv::convertMaps
  *   map1 CV_16SC2 + map2 CV_16UC1 (map2 may be NULL for INTER_NEAREST).  WARP_RELATIVE_MAP is not implemented. */
 B200CV_API int b200cv_remap(const b200cvMat* src, const b200cvMat* dst, const b200cvMat* map1, const b200cvMat* map2, int interpolation,
                             int border, const double* border_value, void* stream);
 /* replace cv::pyrDown / cv::pyrUp (imgproc.hpp:3325, :3351; pyramids.cpp:1348-1400, :1459-1505) for the default destination sizes
- * ((W+1)/2 x (H+1)/2 and 2W x 2H), 8-bit and float, 1/3/4 channels -- SURVEY 8(f) */
+ * ((W+1)/2 x (H+1)/2 and 2W x 2H), 8-bit and float, 1/3/4 channels */
 B200CV_API int b200cv_pyr_down(const b200cvMat* src, const b200cvMat* dst, int border, void* stream);
 B200CV_API int b200cv_pyr_up(const b200cvMat* src, const b200cvMat* dst, int border, void* stream);
 /* replaces cv::cvtColor (imgproc.hpp:3736; color.cpp:192-400) for BGR/RGB(A) <-> GRAY / YUV / YCrCb / HSV(_FULL) / BGR(A), and for the
@@ -199,7 +199,7 @@ B200CV_API int b200cv_cvt_color(const b200cvMat* src, const b200cvMat* dst, int 
  * interleaved chroma plane (8UC2, W/2 x H/2) in separate buffers with their own pitches, as hardware decoders hand them out */
 B200CV_API int b200cv_cvt_color_two_plane(const b200cvMat* src_y, const b200cvMat* src_uv, const b200cvMat* dst, int code, void* stream);
 /* replaces cv::matchTemplate (imgproc.hpp:3916; templmatch.cpp:1158-1194), 1-channel u8/f32, all six methods.
- * result: CV_32FC1 (W-w+1) x (H-h+1).  The CCORR numerator of u8 images runs on tcgen05 tensor cores. */
+ * result: CV_32FC1 (W-w+1) x (H-h+1).  The CCORR numerator of u8 images runs on the tensor cores (wgmma). */
 B200CV_API int b200cv_match_template(const b200cvMat* image, const b200cvMat* templ, const b200cvMat* result,
                                      int method, void* stream);
 /* cv::matchTemplate with a mask (templmatch.cpp:762-905): mask = 8UC1 (non-zero = 1) or 32FC1 (weights) of the template's size, one channel */

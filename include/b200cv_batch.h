@@ -1,5 +1,5 @@
 /*
- * b200cv_batch.h -- the multi-GPU batch driver of the B200 hot path (SURVEY.md section 8(e)).
+ * b200cv_batch.h -- the multi-GPU batch driver of the hot path.
  *
  * A batch of independent frames in HOST memory (cv::Mat layout, b200cvMat with frames > 1) is sharded over the GPUs of one box:
  * frame block [lo, hi) of device i = b200cv_batch_shard (contiguous blocks that differ by at most one frame), one persistent host
@@ -60,7 +60,7 @@ B200CV_API int b200cv_batch_corner_harris(b200cvBatch* batch, const b200cvMat* s
 /* templ: HOST, one frame.  Uploaded to the first device and broadcast to the others (ncclBroadcast), then every worker matches its frames */
 B200CV_API int b200cv_batch_match_template(b200cvBatch* batch, const b200cvMat* image, const b200cvMat* templ, const b200cvMat* result, int method);
 
-/* BASELINE config C5: SIFT Gaussian pyramid + DoG (b200cv_sift_pyramid) and cornerHarris over a sharded batch of 8UC1 host frames, in WAVES
+/* the bench.py c5 workload: SIFT Gaussian pyramid + DoG (b200cv_sift_pyramid) and cornerHarris over a sharded batch of 8UC1 host frames, in WAVES
  * of `wave` frames per device (a 4K frame's pyramids are 1.06 + 0.88 GB: a device holds one wave's pyramids in a reusable arena).
  * harris: HOST CV_32FC1 batch receiving the responses, or NULL (they stay on the device like the pyramids).
  * consumer: NULL, or called on the worker's thread after each wave with DEVICE pointers to that wave's pyramids (layout of b200cv_sift_pyramid,

@@ -1,5 +1,5 @@
 /*
- * b200cv_hal.h -- HOST-pointer entry points of the B200 hot path.
+ * b200cv_hal.h -- HOST-pointer entry points of the hot path.
  *
  * (1) b200cv_hal_*  : exactly the argument lists of the reference's imgproc HAL seam
  *     (modules/imgproc/src/hal_replacement.hpp; each prototype cites the hal_ni_* it replaces), so a stock OpenCV
@@ -8,7 +8,7 @@
  *         #define cv_hal_resize b200cv_hal_resize          (see INTEGRATION.md and hal/b200cv_hal_replacement.hpp)
  *     Calls are synchronous (result in dst on return), thread-safe (per-thread stream + staging buffers), return
  *     CV_HAL_ERROR_OK (0) / CV_HAL_ERROR_NOT_IMPLEMENTED (1: OpenCV silently uses its own code) / other = error
- *     (hal_replacement.hpp:1342-1357).  Inside: H2D copy, the same sm_100a kernels as the device API, D2H copy.
+ *     (hal_replacement.hpp:1342-1357).  Inside: H2D copy, the same sm_90a kernels as the device API, D2H copy.
  *
  * (2) b200cv_host_* : the device API of b200cv.h over HOST b200cvMat descriptors (data = host pointer, ideally
  *     page-locked: b200cv_host_alloc), for BATCHES of frames: frames are cut into chunks that flow through a

@@ -1,4 +1,4 @@
-"""opencv_b200 -- Python face of the B200-native dense-imgproc hot path (libb200cv.so, sm_100a).
+"""opencv_b200 -- Python face of the H100-native dense-imgproc hot path (libb200cv.so, sm_90a).
 
 The functions mirror the cv2 / cv:: names and argument meaning of the reference
 (modules/imgproc/include/opencv2/imgproc.hpp) for the calls on the hot path:
@@ -10,7 +10,7 @@ Inputs are torch CUDA tensors laid out like a cv::Mat -- (H, W) or (H, W, C), or
 (N, H, W[, C]) of independent frames -- and go to the device C ABI (include/b200cv.h) without a
 copy; numpy arrays go through the synchronous host C ABI (include/b200cv_hal.h), which uploads,
 runs the same kernels and downloads.  There is NO CPU fallback: if the CUDA library is missing or
-no B200 is visible every call raises.
+no H100 is visible every call raises.
 """
 import ctypes
 import os

@@ -1,6 +1,6 @@
 """opencv_b200.batch -- sharding a batch of independent frames over the GPUs of one box (one process per GPU).
 
-The hot path has no cross-frame state (SURVEY 8e): rank r owns a contiguous block of frames, runs the whole per-frame
+The hot path has no cross-frame state: rank r owns a contiguous block of frames, runs the whole per-frame
 pipeline on its own stream(s) and keeps its results.  The ONLY exchange is a broadcast of the small shared operand
 (template / filter taps / warp matrix) from rank 0 -- NCCL over NVLink on GPUs, gloo in the CPU tests.
 """
@@ -189,7 +189,7 @@ class BatchDriver:
         return result
 
     def sift_harris(self, src, harris=None, nOctaveLayers=3, sigma=1.6, upscale=1, blockSize=2, ksize=3, k=0.04, wave=4, consumer=None):
-        """BASELINE C5: SIFT pyramid + DoG and cornerHarris over a sharded (N,H,W,1) uint8 batch, `wave` frames per device at a time.
+        """bench.py workload c5: SIFT pyramid + DoG and cornerHarris over a sharded (N,H,W,1) uint8 batch, `wave` frames per device at a time.
         harris: (N,H,W,1) float32 host batch or None.  consumer(device_index, first_frame, n_frames, gauss_ptr, gauss_stride, dog_ptr, dog_stride,
         harris_ptr, harris_step, harris_frame_step) -> 0, called on the worker threads with DEVICE pointers after every wave."""
         ct = self._ct

@@ -1,10 +1,10 @@
 #!/usr/bin/env python3
-"""Build opencv_b200/lib/libb200cv.so (sm_100a only) in-tree with nvcc + g++.
+"""Build opencv_b200/lib/libb200cv.so (sm_90a only) in-tree with nvcc + g++.
 
     python -m opencv_b200.build [-j N] [--force] [--verbose-ptxas]
 
 Every .cu under csrc/ is compiled with
-    nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17
+    nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17
 host-only sources (host_tables.cpp) with g++ -ffp-contract=off (their arithmetic must round exactly like
 the reference's softfloat code), and everything is linked into one shared library with a static cudart.
 """
@@ -21,7 +21,7 @@ OBJ = os.path.join(HERE, "lib", "obj")
 LIB = os.path.join(HERE, "lib", "libb200cv.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC,-fvisibility=hidden,-ffp-contract=off", "--expt-relaxed-constexpr",
               "-I" + os.path.join(HERE, "..", "include")]
 CXX_FLAGS = ["-O2", "-std=c++17", "-fPIC", "-fvisibility=hidden", "-ffp-contract=off",
@@ -51,6 +51,11 @@ def compile_one(src, force, verbose):
 
 def build(jobs=None, force=False, verbose=False):
     os.makedirs(OBJ, exist_ok=True)
+    # objects compiled with other flags (another target architecture) are rebuilt, not linked
+    stamp = os.path.join(OBJ, "flags")
+    flags = " ".join(NVCC_FLAGS + CXX_FLAGS)
+    if not os.path.exists(stamp) or open(stamp).read() != flags:
+        force = True
     srcs = sorted(glob.glob(os.path.join(CSRC, "*.cu")) + glob.glob(os.path.join(CSRC, "*.cpp")))
     objs, failed = [], False
     with cf.ThreadPoolExecutor(max_workers=jobs or os.cpu_count() or 4) as ex:
@@ -68,6 +73,8 @@ def build(jobs=None, force=False, verbose=False):
         if r.returncode != 0:
             sys.stderr.write(r.stdout + r.stderr)
             raise RuntimeError("b200cv: link failed")
+    with open(stamp, "w") as fh:
+        fh.write(flags)
     return LIB
 
 

@@ -1,4 +1,4 @@
-// boxfilter.cu -- cv::boxFilter / cv::blur (SURVEY 8(f) "next": the unweighted member of the separable-filter family).
+// boxfilter.cu -- cv::boxFilter / cv::blur (the unweighted member of the separable-filter family).
 //
 // Reference arithmetic (box_filter.simd.hpp), reproduced per destination element:
 //   8U -> 8U, kw*kh <= 256 ... 16-bit sums, integer divide of ColumnSum<ushort,uchar> (:430-600):

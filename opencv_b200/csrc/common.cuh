@@ -1,4 +1,4 @@
-// common.cuh -- shared device/host helpers for the b200cv kernels (sm_100a only).
+// common.cuh -- shared device/host helpers for the b200cv kernels (sm_90a only).
 #pragma once
 #ifdef B200CV_HOST_EMULATION      // tests/emu/cuda_emu.h: simple kernels compiled for the host by tests/test_kernel_emulation.py
 #include "cuda_emu.h"

@@ -1,4 +1,4 @@
-// cvtcolor_lab.cu -- cv::cvtColor BGR / RGB <-> CIE Lab for 8-bit images (SURVEY 8(f) rank 3): codes 44 BGR2Lab, 45 RGB2Lab, 74 LBGR2Lab,
+// cvtcolor_lab.cu -- cv::cvtColor BGR / RGB <-> CIE Lab for 8-bit images: codes 44 BGR2Lab, 45 RGB2Lab, 74 LBGR2Lab,
 // 75 LRGB2Lab, 56 Lab2BGR, 57 Lab2RGB, 78 Lab2LBGR, 79 Lab2LRGB.
 //
 // The reference's 8-bit paths are integer arithmetic around a handful of tables (color_lab.cpp):

@@ -1,4 +1,4 @@
-// cvtcolor_yuv.cu -- cv::cvtColor for the subsampled-YUV wire formats (SURVEY 8(f) rank 3: what a video decoder hands to the path).
+// cvtcolor_yuv.cu -- cv::cvtColor for the subsampled-YUV wire formats (what a video decoder hands to the path).
 //
 //   4:2:0 two-plane  NV12 / NV21 -> RGB / BGR / RGBA / BGRA       codes 90-97    (color_yuv.simd.hpp:1196-1318)
 //   4:2:0 three-plane YV12 / IYUV -> RGB / BGR / RGBA / BGRA      codes 98-105   (:1320-1448, plane layout :2074-2106)

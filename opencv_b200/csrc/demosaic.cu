@@ -1,5 +1,5 @@
-// demosaic.cu -- cv::cvtColor / cv::demosaicing for the Bayer patterns, bilinear and edge-aware interpolation, 8- and 16-bit (SURVEY 8(f) rank 3:
-// the wire format of a raw sensor).  Codes COLOR_BayerBG/GB/RG/GR2BGR = 46..49 (the 2RGB names are the same numbers permuted), 2BGRA = 139..142,
+// demosaic.cu -- cv::cvtColor / cv::demosaicing for the Bayer patterns, bilinear and edge-aware interpolation, 8- and 16-bit (the
+// wire format of a raw sensor).  Codes COLOR_BayerBG/GB/RG/GR2BGR = 46..49 (the 2RGB names are the same numbers permuted), 2BGRA = 139..142,
 // 2BGR_EA = 135..138.
 //
 // Reference (demosaicing.cpp:806-1056, Bayer2RGB_Invoker / Bayer2RGB_): for every interior pixel of the mosaic

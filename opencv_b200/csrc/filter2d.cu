@@ -213,7 +213,7 @@ extern "C" int b200cv_filter2d(const b200cvMat* src, const b200cvMat* dst, const
             if (rc != B200CV_NOT_IMPLEMENTED) return rc;
         }
     }
-    // float images: same switch point (the reference's DFT regime), 3 x BF16 on tcgen05 with FP32 accumulation (filter2d_tc_f32.cu)
+    // float images: same switch point (the reference's DFT regime), 3 x BF16 on the tensor cores (wgmma) with FP32 accumulation (filter2d_tc_f32.cu)
     if (sd == B200CV_32F && dd == B200CV_32F && cn == 1 && kw * kh >= (tc_min_taps ? tc_min_taps : 130)) {
         const char* path = getenv("B200CV_FILTER2D_PATH");
         if (!(path && !strcmp(path, "direct"))) {

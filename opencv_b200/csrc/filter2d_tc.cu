@@ -1,11 +1,11 @@
-// filter2d_tc.cu -- 8-bit single-channel cv::filter2D with >= 11x11 taps on 5th-generation tensor cores: a persistent,
-// warp-specialised tcgen05 kernel.  (These are the sizes at which the reference itself leaves the direct sum for a DFT,
+// filter2d_tc.cu -- 8-bit single-channel cv::filter2D with >= 11x11 taps on Hopper tensor cores: a persistent, warp-specialised
+// wgmma kernel.  (These are the sizes at which the reference itself leaves the direct sum for a DFT,
 // filter.dispatch.cpp:1288-1310; smaller kernels stay on the FP32 kernel of filter2d_tma.cu.)
 //
 // Arithmetic.  The float taps are quantised to 24-bit fixed point against max|k| (Kq = rint(k 2^sh), |Kq| < 2^22) and split into
 // three balanced base-256 digits d0, d1, d2 in [-128, 127].  With the Toeplitz expansion of matchtemplate_tc.cu,
 //   D_d[m][j] = sum_v sum_k A_v[m][k] * B_{v,d}[k][j],   A_v[m][k] = P(y0+m+v, x0+k),   B_{v,d}[k][j] = d(Kq(v, k-j)),
-// one `kind::i8` MMA (u8 x s8 -> s32, exact) of shape M128 x N96 x K32 carries the three digit planes of a 32-column output tile
+// one integer MMA (u8 x s8 -> s32, exact) of shape M64 x N96 x K32 carries the three digit planes of a 32-column output tile
 // as N = 3 x 32; the epilogue recombines S0 + 256 S1 + 65536 S2 in 64-bit, converts once, scales by 2^-sh and adds delta.  The only
 // error is the tap quantisation (<= 2^-23 max|k| per tap): the same order as a float accumulation, far inside the reference's own
 // tolerance for this path (its DFT).  P is the border-extended image (pad_u8_kernel).
@@ -13,16 +13,18 @@
 // Data movement.  K = 64 per kernel row covers kw <= 33 (kw + 31 <= 64): a kernel row's operand B_v is 4 x 96 x 16 B = 6 KB, so
 // ALL of B (31 rows = 186 KB) stays RESIDENT in shared memory for the life of the CTA.  One CTA per SM walks destination tiles of
 // 256 rows x 32 columns:
-//   warp 0  producer  -- per tile one TMA load of the 64-byte-wide A strip (256 + kh - 1 rows, 18 KB) into a ring of 2-4 buffers
-//   warp 1  issuer    -- kh x 2 M-tiles x 2 K-steps tcgen05.mma per tile into one of two TMEM accumulator stages (2 x 192 columns)
-//   warps 2-9 epilogue -- tcgen05.ld of the previous tile's stage (two warps per TMEM lane quarter, 16 columns each), recombination,
-//                        16-byte row stores, overlapping the next tile's MMAs
-// mbarriers: b_full, a_full/a_empty[2], acc_full/acc_empty[2]; tcgen05.commit releases A buffers and publishes accumulators.
+//   warp 8     producer  -- all of B once, then per tile one TMA load of the 64-byte-wide A strip (256 + kh - 1 rows, 18 KB) into a
+//                           ring of 2-4 buffers
+//   warps 0-7  consumers -- two warpgroups of 128 tile rows each: kh x 2 K-steps x 2 slabs of wgmma m64n96k32 per tile into
+//                           registers, then recombination and stores from the registers; the strip is released before the epilogue,
+//                           so the producer refills it while the warpgroups store
+// mbarriers: b_full, a_full/a_empty[4].
 #include <algorithm>
 #include <cmath>
 #include <cstring>
 #include "common.cuh"
 #include "tma.cuh"
+#include "wgmma.cuh"
 
 namespace b200cv {
 
@@ -31,9 +33,9 @@ void launch_pad_u8(const Img& src, const Img& dst, int ax, int ay, int border, c
 constexpr int FC_NT = 32;                     // output columns per tile
 constexpr int FC_N = 3 * FC_NT;               // MMA N (three digit planes)
 constexpr int FC_K = 64;                      // K per kernel row
-constexpr int FC_MT = 2;                      // M-tiles (128 rows) per tile
+constexpr int FC_WG = 2;                      // consumer warpgroups, 128 tile rows each
 constexpr int FC_BROW = (FC_K / 16) * FC_N * 16;   // bytes of B per kernel row = 6144
-constexpr int FC_THREADS = 320;                // producer warp, issuer warp, 8 epilogue warps
+constexpr int FC_THREADS = 128 * FC_WG + 32;  // consumer warpgroups + one producer warp
 constexpr int FC_SMEM_MAX = 227 * 1024 - 512;   // opt-in limit per CTA (232448 B) minus this kernel's static shared memory (barriers)
 
 struct FCKq { int q[33 * 33]; };
@@ -60,57 +62,6 @@ __global__ void fc_toeplitz_kernel(const __grid_constant__ FCKq kp, int w, signe
     }
 }
 
-__device__ __forceinline__ uint64_t fc_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes)
-{
-    // K-major, no swizzle: start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | version=1 [46,48)
-    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) | (1ull << 46);
-}
-__device__ __forceinline__ void fc_mma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}"
-                 ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// one lane of a converged warp (see matchtemplate_tc.cu: descriptors stay in uniform registers when the issuer loop is warp-uniform)
-__device__ __forceinline__ bool fc_elect_one()
-{
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void fc_commit(uint64_t* bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void fc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fc_bulk_load(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar)
-{
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void fc_mbar_arrive(uint64_t* bar)
-{
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void fc_tmem_ld32(uint32_t taddr, uint32_t* r)
-{
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]),
-          "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]),
-          "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr) : "memory");
-}
-
-__device__ __forceinline__ void fc_tmem_ld16(uint32_t taddr, uint32_t* r)
-{
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]),
-          "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr) : "memory");
-}
-
 enum { FC_U8 = 0, FC_F32 = 1, FC_S16 = 2 };
 
 template <int EPI>
@@ -121,31 +72,22 @@ __global__ void __launch_bounds__(FC_THREADS, 1) filter2d_tc_kernel(const __grid
     const uint32_t abytes = (uint32_t)(FC_K / 16) * p.ra_alloc * 16;        // one A buffer
     unsigned char* sB = smem;                                               // kh x 6 KB, resident
     unsigned char* sA = smem + (size_t)p.kh * FC_BROW;                      // p.na buffers
-    __shared__ __align__(8) uint64_t b_full, a_full[4], a_empty[4], acc_full[2], acc_empty[2];
-    __shared__ uint32_t s_tmem;
+    __shared__ __align__(8) uint64_t b_full, a_full[4], a_empty[4];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t lbo_a = (uint32_t)p.ra_alloc * 16u;
 
     if (threadIdx.x == 0) {
         mbar_init(&b_full, 1);
-        for (int s = 0; s < 4; s++) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 1); }
-        for (int s = 0; s < 2; s++) { mbar_init(&acc_full[s], 1); mbar_init(&acc_empty[s], 8); }
+        for (int s = 0; s < 4; s++) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 4 * FC_WG); }
         fence_barrier_init();
     }
-    if (warp == 1) {   // TMEM: 2 stages x FC_MT x 96 columns of 32-bit accumulators = 384 -> 512 allocated
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)), "r"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    fc_fence_before();
     __syncthreads();
-    fc_fence_after();
-    const uint32_t tmem = s_tmem;
 
-    if (warp == 0) {
+    if (warp == 4 * FC_WG) {
         if (lane == 0) {
             // ---- producer: all of B once, then one A strip per tile ----
             mbar_arrive_expect_tx(&b_full, (uint32_t)p.kh * FC_BROW);
-            for (int v = 0; v < p.kh; v++) fc_bulk_load(sB + (size_t)v * FC_BROW, bglob + (size_t)v * FC_BROW, FC_BROW, &b_full);
+            for (int v = 0; v < p.kh; v++) wg_bulk_load(sB + (size_t)v * FC_BROW, bglob + (size_t)v * FC_BROW, FC_BROW, &b_full);
             int i = 0;
             for (int t = blockIdx.x; t < p.ntiles; t += gridDim.x, i++) {
                 const int tx = t % p.tiles_x, ty = (t / p.tiles_x) % p.tiles_y, f = t / (p.tiles_x * p.tiles_y);
@@ -155,107 +97,72 @@ __global__ void __launch_bounds__(FC_THREADS, 1) filter2d_tc_kernel(const __grid
                 unsigned char* dstA = sA + (size_t)buf * abytes;
                 for (int c = 0; c < FC_K / 16; c++)
                     for (int b = 0; b < p.nbox; b++)
-                        tma_load_3d(dstA + (size_t)c * lbo_a + (size_t)b * p.box_h * 16, &tmap, tx * FC_NT + 16 * c, ty * (128 * FC_MT) + b * p.box_h, f, &a_full[buf]);
+                        tma_load_3d(dstA + (size_t)c * lbo_a + (size_t)b * p.box_h * 16, &tmap, tx * FC_NT + 16 * c, ty * (128 * FC_WG) + b * p.box_h, f, &a_full[buf]);
             }
         }
-    } else if (warp == 1) {
-        // ---- MMA issuer: the whole warp runs the loops (uniform values), one elected lane issues ----
-        // instruction descriptor: D = S32 (2<<4), A = u8 (0 at [7,10)), B = s8 (1 at [10,13)), K-major both, N>>3 at [17,23), M>>4 at [24,29)
-        const uint32_t idesc = (2u << 4) | (1u << 10) | ((uint32_t)(FC_N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-        mbar_wait(&b_full, 0);
-        // descriptors (K-major, no swizzle): low word = start >> 4 [0,14) | LBO >> 4 [16,30); high word = SBO >> 4 | version 1 at bit 14
-        const uint32_t hi = (128u >> 4) | (1u << 14);
-        const uint32_t b_lo0 = ((smem_u32(sB) & 0x3FFFFu) >> 4) | (((uint32_t)(FC_N * 16) >> 4) << 16);
-        const uint32_t a_ks = (2u * lbo_a) >> 4;
-        int i = 0;
-        for (int t = blockIdx.x; t < p.ntiles; t += gridDim.x, i++) {
-            const int buf = i % p.na, acc = i & 1;
-            mbar_wait(&a_full[buf], (i / p.na) & 1);
-            mbar_wait(&acc_empty[acc], ((i >> 1) & 1) ^ 1);
-            fc_fence_after();
-            const uint32_t a_lo0 = ((smem_u32(sA + (size_t)buf * abytes) & 0x3FFFFu) >> 4) | ((lbo_a >> 4) << 16);
-            const uint32_t d_base = tmem + (uint32_t)acc * (FC_MT * FC_N);
-            if (fc_elect_one()) {
+        return;
+    }
+
+    // ---- consumers: warpgroup wg owns tile rows 128 wg .. 128 wg + 127 as two 64-row slabs; per tile kh x 2 K-steps x 2 slabs of
+    //      wgmma m64n96k32, then the epilogue from the registers while the other warpgroup / the next strip keep the pipe busy ----
+    const int wg = warp >> 2, wl = warp & 3;
+    mbar_wait(&b_full, 0);
+    const uint32_t b0 = smem_u32(sB);
+    int i = 0;
+    for (int t = blockIdx.x; t < p.ntiles; t += gridDim.x, i++) {
+        const int tx = t % p.tiles_x, ty = (t / p.tiles_x) % p.tiles_y, f = t / (p.tiles_x * p.tiles_y);
+        const int buf = i % p.na;
+        uint32_t acc[2][FC_N / 2];
+#pragma unroll
+        for (int m = 0; m < 2; m++)
+#pragma unroll
+            for (int r = 0; r < FC_N / 2; r++) acc[m][r] = 0;
+        mbar_wait(&a_full[buf], (i / p.na) & 1);
+        wg_fence();
+        const uint32_t a0 = smem_u32(sA + (size_t)buf * abytes) + (uint32_t)(wg * 128) * 16u;
 #pragma unroll 1
-                for (int v = 0; v < p.kh; v++) {
+        for (int v = 0; v < p.kh; v++) {
 #pragma unroll
-                    for (int mt = 0; mt < FC_MT; mt++)
+            for (int ks = 0; ks < FC_K / 32; ks++) {
+                const uint64_t bd = wg_desc(b0 + (uint32_t)v * FC_BROW + (uint32_t)ks * (2 * FC_N * 16), FC_N * 16, 128);
 #pragma unroll
-                        for (int ks = 0; ks < FC_K / 32; ks++) {
-                            const uint64_t ad = ((uint64_t)hi << 32) | (a_lo0 + (uint32_t)ks * a_ks + (uint32_t)(mt * 128 + v));
-                            const uint64_t bd = ((uint64_t)hi << 32) | (b_lo0 + (uint32_t)v * (FC_BROW >> 4) + (uint32_t)ks * ((2u * FC_N * 16) >> 4));
-                            fc_mma(d_base + mt * FC_N, ad, bd, idesc, (v | ks) != 0);
-                        }
-                }
-                fc_commit(&a_empty[buf]);        // the A strip may be overwritten once these MMAs have read it
-                fc_commit(&acc_full[acc]);       // ... and the accumulator stage is complete
+                for (int m = 0; m < 2; m++)    // kernel row v: the same strip, v rows further down
+                    wgmma_u8s8_n96(acc[m], wg_desc(a0 + (uint32_t)ks * 2u * lbo_a + (uint32_t)(m * 64 + v) * 16u, lbo_a, 128), bd);
             }
-            __syncwarp();
         }
-    } else {
-        // ---- epilogue: warps 2..9; warp w may touch TMEM lanes 32 (w % 4) .. +31 = accumulator rows; the two warps of a quarter
-        //      split the 32 output columns ----
-        const int quarter = warp & 3, half = (warp - 2) >> 2;
-        int i = 0;
-        for (int t = blockIdx.x; t < p.ntiles; t += gridDim.x, i++) {
-            const int tx = t % p.tiles_x, ty = (t / p.tiles_x) % p.tiles_y, f = t / (p.tiles_x * p.tiles_y);
-            const int buf = i & 1;
-            mbar_wait(&acc_full[buf], (i >> 1) & 1);
-            fc_fence_after();
-            const int gx0 = tx * FC_NT + half * 16;
-#pragma unroll 1
-            for (int mt = 0; mt < FC_MT; mt++) {
-                const int gy = ty * (128 * FC_MT) + mt * 128 + quarter * 32 + lane;
-                const uint32_t trow = tmem + ((uint32_t)(quarter * 32) << 16) + (uint32_t)buf * (FC_MT * FC_N) + mt * FC_N + half * 16;
-                uint32_t r0[16], r1[16], r2[16];
-                fc_tmem_ld16(trow, r0);
-                fc_tmem_ld16(trow + FC_NT, r1);
-                fc_tmem_ld16(trow + 2 * FC_NT, r2);
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                float v[16];
+        wg_commit();
+        wg_wait<0>();
+        wg_fence_operand(acc[0]);
+        wg_fence_operand(acc[1]);
+        wg_mbar_arrive_if(&a_empty[buf], lane == 0);          // 8 arrivals (one per consumer warp) free the strip
+        // ---- epilogue: column jj of the tile has its digit sums at N = jj, 32 + jj, 64 + jj ----
 #pragma unroll
-                for (int j = 0; j < 16; j++) {
-                    const long long sum = (long long)(int)r0[j] + ((long long)(int)r1[j] << 8) + ((long long)(int)r2[j] << 16);
-                    v[j] = __fadd_rn(__fmul_rn(__ll2float_rn(sum), p.scale), p.delta);
-                }
-                if (gy < p.oh && gx0 < p.ow) {
-                    if constexpr (EPI == FC_U8) {
-                        uchar* dp = dst.row<uchar>(f, gy) + gx0;
-                        if (gx0 + 16 <= p.ow && ((uintptr_t)dp & 15) == 0) {
-                            uint32_t w[4];
+        for (int m = 0; m < 2; m++)
 #pragma unroll
-                            for (int j = 0; j < 4; j++)
-                                w[j] = (uint32_t)sat_u8(v[4 * j]) | ((uint32_t)sat_u8(v[4 * j + 1]) << 8) | ((uint32_t)sat_u8(v[4 * j + 2]) << 16) |
-                                       ((uint32_t)sat_u8(v[4 * j + 3]) << 24);
-                            *(uint4*)dp = make_uint4(w[0], w[1], w[2], w[3]);
-                        } else {
+            for (int ii = 0; ii < 2; ii++) {
+                const int gy = ty * (128 * FC_WG) + wg * 128 + m * 64 + wl * 16 + (lane >> 2) + 8 * ii;
+                if (gy >= p.oh) continue;
 #pragma unroll
-                            for (int j = 0; j < 16; j++) if (gx0 + j < p.ow) dp[j] = sat_u8(v[j]);
-                        }
-                    } else if constexpr (EPI == FC_S16) {
-                        short* dp = dst.row<short>(f, gy) + gx0;
+                for (int j = 0; j < FC_NT / 8; j++) {
+                    const int gx = tx * FC_NT + 8 * j + 2 * (lane & 3);
+                    float v[2];
 #pragma unroll
-                        for (int j = 0; j < 16; j++) if (gx0 + j < p.ow) dp[j] = sat_s16(v[j]);
-                    } else {
-                        float* dp = dst.row<float>(f, gy) + gx0;
-                        if (gx0 + 16 <= p.ow && ((uintptr_t)dp & 15) == 0) {
+                    for (int c = 0; c < 2; c++) {
+                        const int r = 4 * j + 2 * ii + c;
+                        const long long sum = (long long)(int)acc[m][r] + ((long long)(int)acc[m][r + FC_NT / 2] << 8) +
+                                              ((long long)(int)acc[m][r + FC_NT] << 16);
+                        v[c] = __fadd_rn(__fmul_rn(__ll2float_rn(sum), p.scale), p.delta);
+                    }
 #pragma unroll
-                            for (int j = 0; j < 4; j++) ((float4*)dp)[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-                        } else {
-#pragma unroll
-                            for (int j = 0; j < 16; j++) if (gx0 + j < p.ow) dp[j] = v[j];
-                        }
+                    for (int c = 0; c < 2; c++) {
+                        if (gx + c >= p.ow) continue;
+                        if constexpr (EPI == FC_U8) dst.row<uchar>(f, gy)[gx + c] = sat_u8(v[c]);
+                        else if constexpr (EPI == FC_S16) dst.row<short>(f, gy)[gx + c] = sat_s16(v[c]);
+                        else dst.row<float>(f, gy)[gx + c] = v[c];
                     }
                 }
             }
-            fc_fence_before();
-            __syncwarp();
-            if (lane == 0) fc_mbar_arrive(&acc_empty[buf]);      // 8 arrivals (one per epilogue warp) free the stage
-        }
     }
-    fc_fence_before();
-    __syncthreads();
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512) : "memory");
 }
 
 template <int EPI>
@@ -292,11 +199,11 @@ int filter2d_u8_tensor(const Img& s, const Img& d, int dd, const float* k, int k
     FCParams p;
     memset(&p, 0, sizeof(p));
     p.kh = kh; p.ow = s.cols; p.oh = s.rows; p.frames = s.frames; p.scale = (float)std::ldexp(1.0, -sh); p.delta = delta;
-    p.tiles_x = (int)div_up((unsigned)p.ow, FC_NT); p.tiles_y = (int)div_up((unsigned)p.oh, 128 * FC_MT);
+    p.tiles_x = (int)div_up((unsigned)p.ow, FC_NT); p.tiles_y = (int)div_up((unsigned)p.oh, 128 * FC_WG);
     const long long nt = (long long)p.tiles_x * p.tiles_y * p.frames;
     if (nt > 0x7fffffff) return B200CV_NOT_IMPLEMENTED;
     p.ntiles = (int)nt;
-    const int ra = 128 * FC_MT + kh - 1;
+    const int ra = 128 * FC_WG + kh - 1;
     p.nbox = (ra + 255) / 256;
     p.box_h = (((ra + p.nbox - 1) / p.nbox) + 7) & ~7;
     p.ra_alloc = p.nbox * p.box_h;

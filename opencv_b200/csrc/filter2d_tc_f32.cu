@@ -1,35 +1,32 @@
-// filter2d_tc_f32.cu -- float single-channel cv::filter2D with >= 130 taps on 5th-generation tensor cores (tcgen05, kind::f16 with
-// BF16 operands and FP32 accumulators in TMEM): exactly the sizes at which the reference leaves its direct sum for a float DFT
+// filter2d_tc_f32.cu -- float single-channel cv::filter2D with >= 130 taps on Hopper tensor cores (wgmma with BF16 operands and FP32
+// accumulators in registers): exactly the sizes at which the reference leaves its direct sum for a float DFT
 // (dft_filter_size, filter.dispatch.cpp:1288-1290; its own tolerance there is 1e-4 of the value range, test_filter.cpp:420-425).
 // Smaller kernels stay on the FP32 kernel of filter2d_tma.cu, which reproduces the reference's direct sum bit for bit.
 //
 // Arithmetic: 3 x BF16.  Every float is split into hi = bf16(a) and lo = bf16(a - hi) (|a - hi - lo| <= 2^-16 |a|); the product sum is
 //   sum a k  ~=  sum a_hi k_hi + sum a_hi k_lo + sum a_lo k_hi        (the dropped a_lo k_lo term is another 2^-16)
-// three MMAs into ONE FP32 accumulator.  Relative to sum |a| |k| the error is <= ~4e-5 worst case (all signs aligned), ~1e-6 typical --
-// inside the reference's bar for this regime and below what its float DFT itself loses on 31 x 31 kernels.  BF16 keeps float's exponent
-// range, so no data-dependent scaling (and no reduction pass over the image) is needed.
+// in FP32 accumulators.  Relative to sum |a| |k| the error is <= ~4e-5 worst case (all signs aligned), ~1e-6 typical -- inside the
+// reference's bar for this regime and below what its float DFT itself loses on 31 x 31 kernels.  BF16 keeps float's exponent range, so
+// no data-dependent scaling (and no reduction pass over the image) is needed.
 //
 // Contraction = the Toeplitz form of filter2d_tc.cu / matchtemplate_tc.cu:
 //   D[m][j] = sum_v sum_k A_v[m][k] * B_v[k][j],   A_v[m][k] = P(y0 + m + v, x0 + k),   B_v[k][j] = K(v, k - j)   (0 outside 0 <= k-j < kw)
-// with P the border-extended image.  Tile = 256 rows x 32 columns (two M128 accumulators), K = kw + 31 rounded up to 16.
+// with P the border-extended image.  Tile = 256 rows x 32 columns, K = kw + 31 rounded up to 16.
 //
-// What bounds it (profiles/r02_prof_filter2d_tc_f32_before_ncu_full_summary.txt): the first version used N = 16 tiles and three N16 MMAs per
-// K step; the tensor pipe was active 20 % of the time while l1tex__data_pipe_tc_wavefronts_mem_shared sat at 90 % of peak -- every
-// tcgen05.mma re-reads its M128 x K16 BF16 A operand (4 KB = 32 cycles of shared-memory bandwidth) whatever N is, so an N16 MMA costs ~40
-// cycles for 8 cycles of math.  This version amortises the A reads: per K step TWO MMAs instead of three,
+// Every MMA reads its whole A operand from shared memory whatever N is, so the A reads are amortised over N: per K step and 64-row
+// slab TWO MMAs instead of three,
 //     D[:, 0:64)  += A_hi x [B_hi | B_lo]      (N = 64: the hi and lo Toeplitz planes side by side in N)
-//     D[:, 0:32)  += A_lo x  B_hi              (N = 32: the same operand, first half)
-// and the epilogue adds the two column groups.  Per output column and kernel row that is ~11 cycles of operand traffic instead of ~25.
-// The Toeplitz operands no longer fit shared memory for 31 rows (8 KB per kernel row): they stream through a ring from L2 (16 B/clk/SM).
+//     E[:, 0:32)  += A_lo x  B_hi              (N = 32: the same operand, first half)
+// and the epilogue adds D[:, j] + E[:, j] + D[:, 32 + j].
+// The Toeplitz operands do not fit shared memory for 31 rows (8 KB per kernel row): they stream through a ring from L2.
 //
-// Roles (384 threads, one persistent CTA per SM):
-//   warp 0      A producer: per tile the hi and lo strips (K columns x 256 + kh - 1 rows) by TMA in the K-major no-swizzle core-matrix
+// Roles (320 threads, one persistent CTA per SM):
+//   warp 8      A producer: per tile the hi and lo strips (K columns x 256 + kh - 1 rows) by TMA in the K-major no-swizzle core-matrix
 //               layout (one 16-byte-wide box column per 8 K elements), ring of 2 stages
-//   warp 1      B producer: one kernel row of Toeplitz operands (8 KB) per cp.async.bulk into a ring of 4, in the order the issuers use them
-//   warps 2-3   MMA issuers, one per M-tile: kh x K/16 x 2 tcgen05.mma per tile; a kernel row's A operand is the same strip with the
-//               descriptor start address advanced by one 16-byte row; descriptors are a 32-bit add on the low word, the K loop is unrolled
-//               by template, the warp runs the loops uniformly and an elected lane issues; tcgen05.commit frees the B stage per kernel row
-//   warps 4-11  epilogue: tcgen05.ld of the other accumulator stage (64 columns), group 0 + group 1 + delta, 128-byte row stores
+//   warp 9      B producer: one kernel row of Toeplitz operands (8 KB) per cp.async.bulk into a ring of 4, in the order the consumers use them
+//   warps 0-7   two consumer warpgroups of 128 tile rows each: kh x K/16 x 2 slabs x 2 wgmma per tile; a kernel row's A operand is the
+//               same strip with the descriptor start address advanced by one 16-byte row; a B stage is released as soon as the next kernel
+//               row's MMAs are in flight; the epilogue stores from the registers
 // The border-extended BF16 planes are written once per call by pad_split_kernel (reads 4 B, writes 4 B per pixel).
 #include <algorithm>
 #include <cmath>
@@ -38,12 +35,13 @@
 #include <cuda_bf16.h>
 #include "common.cuh"
 #include "tma.cuh"
+#include "wgmma.cuh"
 
 namespace b200cv {
 
 constexpr int FF_N = 32;                      // output columns per tile; the MMAs are N = 64 (hi | lo Toeplitz planes) and N = 32 (hi)
-constexpr int FF_MT = 2;                      // M-tiles (128 rows) per tile
-constexpr int FF_THREADS = 32 * (2 + FF_MT + 8);   // A producer, B producer, 2 issuers, 8 epilogue warps
+constexpr int FF_WG = 2;                      // consumer warpgroups, 128 tile rows each
+constexpr int FF_THREADS = 128 * FF_WG + 64;  // consumer warpgroups, A producer warp, B producer warp
 constexpr int FF_SMEM_MAX = 227 * 1024 - 1024;
 constexpr int FF_NA = 2;                      // A stages
 constexpr int FF_NB = 4;                      // B stages (kernel rows in flight)
@@ -76,7 +74,7 @@ __global__ void ff_toeplitz_kernel(const __grid_constant__ FFTaps kp, int kw, in
 
 // border-extended source as two BF16 planes: out[pl][f][y][x] = split(src(border(y - ay), border(x - ax))).  One thread = 8 adjacent
 // elements of a row (pw is a multiple of 8): two 16-byte stores; the border rule per element only in the strips that leave the image
-// (the first version, one element and two 2-byte stores per thread, took 0.23 ms for 8 4K frames -- a third of the whole op).
+// (the first version wrote one element and two 2-byte stores per thread).
 __global__ void __launch_bounds__(128) ff_pad_split_kernel(Img src, __nv_bfloat16* out, int pw, int ph, int ax, int ay, int border, size_t plane_elems)
 {
     const int x0 = (blockIdx.x * blockDim.x + threadIdx.x) * 8, y = blockIdx.y, f = blockIdx.z;
@@ -108,55 +106,6 @@ __global__ void __launch_bounds__(128) ff_pad_split_kernel(Img src, __nv_bfloat1
     *(uint4*)(out + plane_elems + o) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
 }
 
-__device__ __forceinline__ uint64_t ff_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes)
-{
-    // K-major, no swizzle: start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | version=1 [46,48)
-    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) | (1ull << 46);
-}
-__device__ __forceinline__ void ff_mma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                 ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// one lane of a converged warp (elect.sync): the MMA issuers run their loops warp-uniformly and elect the thread that issues, so the
-// descriptors live in uniform registers (under `if (lane == 0)` every operand went through an R2UR waterfall loop: ~15 instructions per MMA)
-__device__ __forceinline__ bool ff_elect_one()
-{
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void ff_commit(uint64_t* bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void ff_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void ff_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void ff_bulk_load(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar)
-{
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void ff_mbar_arrive(uint64_t* bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory"); }
-__device__ __forceinline__ void ff_tmem_ld16(uint32_t taddr, uint32_t* r)
-{
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]),
-          "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr) : "memory");
-}
-
-__device__ __forceinline__ void ff_tmem_ld32(uint32_t taddr, uint32_t* r)
-{
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]),
-          "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr) : "memory");
-}
-
 template <int KS>      // K / 16: MMA steps per kernel row
 __global__ void __launch_bounds__(FF_THREADS, 1) filter2d_tc_f32_kernel(const __grid_constant__ CUtensorMap tmap, const unsigned char* __restrict__ bglob,
                                                                         Img dst, const __grid_constant__ FFParams p)
@@ -169,28 +118,17 @@ __global__ void __launch_bounds__(FF_THREADS, 1) filter2d_tc_f32_kernel(const __
     const uint32_t abytes = 2 * aplane;                                      // one A stage (hi + lo)
     unsigned char* sB = smem;                                                // FF_NB stages of one kernel row
     unsigned char* sA = smem + (size_t)FF_NB * brow;                         // FF_NA stages
-    __shared__ __align__(8) uint64_t b_full[FF_NB], b_empty[FF_NB], a_full[FF_NA], a_empty[FF_NA], acc_full[2][FF_MT], acc_empty[2][FF_MT];
-    __shared__ uint32_t s_tmem;
+    __shared__ __align__(8) uint64_t b_full[FF_NB], b_empty[FF_NB], a_full[FF_NA], a_empty[FF_NA];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    constexpr int TM_COLS = 2 * FF_MT * 2 * FF_N;                            // 2 stages x M-tiles x 64 columns = 256
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < FF_NB; s++) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], FF_MT); }
-        for (int s = 0; s < FF_NA; s++) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], FF_MT); }
-        for (int s = 0; s < 2; s++)
-            for (int m = 0; m < FF_MT; m++) { mbar_init(&acc_full[s][m], 1); mbar_init(&acc_empty[s][m], 4); }
+        for (int s = 0; s < FF_NB; s++) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], 4 * FF_WG); }
+        for (int s = 0; s < FF_NA; s++) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 4 * FF_WG); }
         fence_barrier_init();
     }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)), "r"(TM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    ff_fence_before();
     __syncthreads();
-    ff_fence_after();
-    const uint32_t tmem = s_tmem;
 
-    if (warp == 0) {
+    if (warp == 4 * FF_WG) {
         if (lane == 0) {
             // ---- A producer: the hi + lo strips of every tile ----
             int i = 0;
@@ -204,108 +142,88 @@ __global__ void __launch_bounds__(FF_THREADS, 1) filter2d_tc_f32_kernel(const __
                     for (int c = 0; c < KCH; c++)
                         for (int b = 0; b < p.nbox; b++)
                             tma_load_3d(dstA + (size_t)pl * aplane + (size_t)c * lbo_a + (size_t)b * p.box_h * 16, &tmap, tx * FF_N + 8 * c,
-                                        ty * (128 * FF_MT) + b * p.box_h, f + pl * p.frames, &a_full[buf]);
+                                        ty * (128 * FF_WG) + b * p.box_h, f + pl * p.frames, &a_full[buf]);
             }
         }
-    } else if (warp == 1) {
+        return;
+    }
+    if (warp == 4 * FF_WG + 1) {
         if (lane == 0) {
-            // ---- B producer: kernel row after kernel row, tile after tile, in the issuers' order ----
+            // ---- B producer: kernel row after kernel row, tile after tile, in the consumers' order ----
             int g = 0;
             for (int t = blockIdx.x; t < p.ntiles; t += gridDim.x)
                 for (int v = 0; v < p.kh; v++, g++) {
                     const int s = g % FF_NB;
                     mbar_wait(&b_empty[s], ((g / FF_NB) & 1) ^ 1);
                     mbar_arrive_expect_tx(&b_full[s], brow);
-                    ff_bulk_load(sB + (size_t)s * brow, bglob + (size_t)v * brow, brow, &b_full[s]);
+                    wg_bulk_load(sB + (size_t)s * brow, bglob + (size_t)v * brow, brow, &b_full[s]);
                 }
         }
-    } else if (warp < 2 + FF_MT) {
-        // ---- MMA issuer of M-tile mt.  The whole warp runs the loops (uniform values), one elected lane issues ----
-        const int mt = __shfl_sync(0xffffffffu, warp, 0) - 2;
-        // instruction descriptor: D = F32 (1 << 4), A = B = BF16 (1 at [7,10) and [10,13)), K-major both, N >> 3 at [17,23), M >> 4 at [24,29)
-        const uint32_t idesc_base = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(128 >> 4) << 24);
-        const uint32_t idesc64 = idesc_base | ((uint32_t)((2 * FF_N) >> 3) << 17), idesc32 = idesc_base | ((uint32_t)(FF_N >> 3) << 17);
-        // shared-memory descriptors (K-major, no swizzle): low word = start >> 4 [0,14) | LBO >> 4 [16,30); high word = SBO >> 4 [0,14) | version 1 at bit 14.
-        // Everything that changes from MMA to MMA is the start address: a 32-bit add on the low word.
-        const uint32_t hi = (128u >> 4) | (1u << 14);
-        const uint32_t a_lbo = (lbo_a >> 4) << 16, b_lbo = ((uint32_t)(2 * FF_N * 16) >> 4) << 16;
-        const uint32_t a_ks = (2u * lbo_a) >> 4, a_pl = aplane >> 4;                // per K step / hi -> lo plane
-        constexpr uint32_t b_ks = (2u * 2 * FF_N * 16) >> 4;
-        const uint32_t b_base = (smem_u32(sB) & 0x3FFFFu) >> 4;
-        int i = 0, g = 0;
-        for (int t = blockIdx.x; t < p.ntiles; t += gridDim.x, i++) {
-            const int buf = i % FF_NA, acc = i & 1;
-            mbar_wait(&a_full[buf], (i / FF_NA) & 1);
-            mbar_wait(&acc_empty[acc][mt], ((i >> 1) & 1) ^ 1);
-            ff_fence_after();
-            const uint32_t d_addr = tmem + (uint32_t)(acc * FF_MT + mt) * (2 * FF_N);
-            uint32_t a_lo = ((smem_u32(sA + (size_t)buf * abytes) + (uint32_t)(mt * 128) * 16u) & 0x3FFFFu) >> 4 | a_lbo;      // + v rows
-#pragma unroll 1
-            for (int v = 0; v < p.kh; v++, g++, a_lo++) {
-                const int s = g % FF_NB;
-                mbar_wait(&b_full[s], (g / FF_NB) & 1);
-                ff_fence_after();
-                if (ff_elect_one()) {
-                    const uint32_t b_lo = (b_base + (uint32_t)s * (brow >> 4)) | b_lbo;
-#pragma unroll
-                    for (int ks = 0; ks < KS; ks++) {
-                        const uint64_t ah = ((uint64_t)hi << 32) | (a_lo + ks * a_ks), al = ((uint64_t)hi << 32) | (a_lo + ks * a_ks + a_pl);
-                        const uint64_t bd = ((uint64_t)hi << 32) | (b_lo + ks * b_ks);
-                        ff_mma(d_addr, ah, bd, idesc64, (v == 0 && ks == 0) ? 0u : 1u);      // A_hi x [B_hi | B_lo] -> columns 0..63
-                        ff_mma(d_addr, al, bd, idesc32, 1u);                                  // A_lo x B_hi        -> columns 0..31
-                    }
-                    ff_commit(&b_empty[s]);        // both issuers arrive: the B stage may be overwritten once their MMAs have read it
-                }
-                __syncwarp();
-            }
-            if (ff_elect_one()) {
-                ff_commit(&a_empty[buf]);          // both issuers arrive: the strip may be overwritten once their MMAs have read it
-                ff_commit(&acc_full[acc][mt]);
-            }
-            __syncwarp();
-        }
-    } else {
-        // ---- epilogue: warps 4..11; a warp may touch TMEM lanes 32 (warp % 4) .. +31 = accumulator rows; four warps per M-tile ----
-        const int quarter = warp & 3, mt = (warp - 2 - FF_MT) >> 2;
-        int i = 0;
-        for (int t = blockIdx.x; t < p.ntiles; t += gridDim.x, i++) {
-            const int tx = t % p.tiles_x, ty = (t / p.tiles_x) % p.tiles_y, f = t / (p.tiles_x * p.tiles_y);
-            const int acc = i & 1;
-            mbar_wait(&acc_full[acc][mt], (i >> 1) & 1);
-            ff_fence_after();
-            const int gx0 = tx * FF_N;
-            const int gy = ty * (128 * FF_MT) + mt * 128 + quarter * 32 + lane;
-            uint32_t r0[32], r1[32];
-            const uint32_t taddr = tmem + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * FF_MT + mt) * (2 * FF_N);
-            ff_tmem_ld32(taddr, r0);
-            ff_tmem_ld32(taddr + FF_N, r1);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            ff_fence_before();
-            __syncwarp();
-            if (lane == 0) ff_mbar_arrive(&acc_empty[acc][mt]);       // 4 arrivals free the accumulators: the values are in registers
-            if (gy < p.oh) {
-                float* dp = dst.row<float>(f, gy) + gx0;
-                if (gx0 + FF_N <= p.ow && ((uintptr_t)dp & 15) == 0) {
-#pragma unroll
-                    for (int j = 0; j < FF_N / 4; j++) {
-                        float4 o;
-                        o.x = __fadd_rn(__fadd_rn(__uint_as_float(r0[4 * j]), __uint_as_float(r1[4 * j])), p.delta);
-                        o.y = __fadd_rn(__fadd_rn(__uint_as_float(r0[4 * j + 1]), __uint_as_float(r1[4 * j + 1])), p.delta);
-                        o.z = __fadd_rn(__fadd_rn(__uint_as_float(r0[4 * j + 2]), __uint_as_float(r1[4 * j + 2])), p.delta);
-                        o.w = __fadd_rn(__fadd_rn(__uint_as_float(r0[4 * j + 3]), __uint_as_float(r1[4 * j + 3])), p.delta);
-                        ((float4*)dp)[j] = o;
-                    }
-                } else {
-#pragma unroll
-                    for (int j = 0; j < FF_N; j++)
-                        if (gx0 + j < p.ow) dp[j] = __fadd_rn(__fadd_rn(__uint_as_float(r0[j]), __uint_as_float(r1[j])), p.delta);
-                }
-            }
-        }
+        return;
     }
-    ff_fence_before();
-    __syncthreads();
-    if (warp == 2) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(TM_COLS) : "memory");
+
+    // ---- consumers: warpgroup wg owns tile rows 128 wg .. 128 wg + 127 as two 64-row slabs ----
+    const int wg = warp >> 2, wl = warp & 3;
+    const uint32_t b_base = smem_u32(sB);
+    int i = 0, g = 0;
+    for (int t = blockIdx.x; t < p.ntiles; t += gridDim.x, i++) {
+        const int tx = t % p.tiles_x, ty = (t / p.tiles_x) % p.tiles_y, f = t / (p.tiles_x * p.tiles_y);
+        const int buf = i % FF_NA;
+        float acc[2][FF_N], alo[2][FF_N / 2];        // A_hi x [B_hi | B_lo] (64 columns) and A_lo x B_hi (32 columns)
+#pragma unroll
+        for (int m = 0; m < 2; m++) {
+#pragma unroll
+            for (int r = 0; r < FF_N; r++) acc[m][r] = 0.f;
+#pragma unroll
+            for (int r = 0; r < FF_N / 2; r++) alo[m][r] = 0.f;
+        }
+        mbar_wait(&a_full[buf], (i / FF_NA) & 1);
+        wg_fence();
+        const uint32_t a0 = smem_u32(sA + (size_t)buf * abytes) + (uint32_t)(wg * 128) * 16u;
+        int prev = -1;
+#pragma unroll 1
+        for (int v = 0; v < p.kh; v++, g++) {
+            const int s = g % FF_NB;
+            mbar_wait(&b_full[s], (g / FF_NB) & 1);
+#pragma unroll
+            for (int ks = 0; ks < KS; ks++) {
+                const uint64_t bd = wg_desc(b_base + (uint32_t)s * brow + (uint32_t)ks * (2 * 2 * FF_N * 16), 2 * FF_N * 16, 128);
+#pragma unroll
+                for (int m = 0; m < 2; m++) {       // kernel row v: the same strip, v rows further down
+                    const uint32_t a = a0 + (uint32_t)ks * 2u * lbo_a + (uint32_t)(m * 64 + v) * 16u;
+                    wgmma_bf16_n64(acc[m], wg_desc(a, lbo_a, 128), bd);
+                    wgmma_bf16_n32(alo[m], wg_desc(a + aplane, lbo_a, 128), bd);
+                }
+            }
+            wg_commit();
+            wg_wait<1>();                            // the previous kernel row's MMAs are done: its B stage may be refilled
+            wg_mbar_arrive_if(&b_empty[prev < 0 ? 0 : prev], lane == 0 && prev >= 0);
+            prev = s;
+        }
+        wg_wait<0>();
+        wg_fence_operand(acc[0]);
+        wg_fence_operand(acc[1]);
+        wg_fence_operand(alo[0]);
+        wg_fence_operand(alo[1]);
+        wg_mbar_arrive_if(&b_empty[prev], lane == 0);
+        wg_mbar_arrive_if(&a_empty[buf], lane == 0);
+        // ---- epilogue: hi x hi + lo x hi + hi x lo + delta ----
+#pragma unroll
+        for (int m = 0; m < 2; m++)
+#pragma unroll
+            for (int ii = 0; ii < 2; ii++) {
+                const int gy = ty * (128 * FF_WG) + wg * 128 + m * 64 + wl * 16 + (lane >> 2) + 8 * ii;
+                if (gy >= p.oh) continue;
+                float* dp = dst.row<float>(f, gy);
+#pragma unroll
+                for (int j = 0; j < FF_N / 8; j++)
+#pragma unroll
+                    for (int c = 0; c < 2; c++) {
+                        const int gx = tx * FF_N + 8 * j + 2 * (lane & 3) + c, r = 4 * j + 2 * ii + c;
+                        if (gx < p.ow) dp[gx] = __fadd_rn(__fadd_rn(__fadd_rn(acc[m][r], alo[m][r]), acc[m][r + FF_N / 2]), p.delta);
+                    }
+            }
+    }
 }
 
 // filter2D, float single-channel source and destination.
@@ -313,8 +231,9 @@ __global__ void __launch_bounds__(FF_THREADS, 1) filter2d_tc_f32_kernel(const __
 int filter2d_f32_tensor(const Img& s, const Img& d, const float* k, int kw, int kh, int ax, int ay, float delta, int border, cudaStream_t st)
 {
     if (kw > 33 || kh > 33 || s.frames >= 32768) return B200CV_NOT_IMPLEMENTED;
-    // the cost grows with the kernel ROWS whatever the width: below 13 rows the direct FP32 sum is at least as fast (DESIGN.md section 5)
-    if (kh < 13 && !getenv("B200CV_FILTER2D_TC_MIN_TAPS")) return B200CV_NOT_IMPLEMENTED;
+    // the cost grows with the kernel ROWS whatever the width: below 14 rows the direct FP32 sum is faster.  Measured on an H100 80GB HBM3
+    // (700 W) with tools/f2d_rows_switch.py, 8 4K frames: 13 x 11 taps 0.73 ms direct / 0.87 ms here, 15 x 9 taps 1.11 / 1.03 ms.
+    if (kh < 14 && !getenv("B200CV_FILTER2D_TC_MIN_TAPS")) return B200CV_NOT_IMPLEMENTED;
     static thread_local FFTaps taps;
     for (int i = 0; i < kw * kh; i++) {
         if (!std::isfinite(k[i])) return B200CV_NOT_IMPLEMENTED;
@@ -324,11 +243,11 @@ int filter2d_f32_tensor(const Img& s, const Img& d, const float* k, int kw, int 
     memset(&p, 0, sizeof(p));
     p.kh = kh; p.ow = s.cols; p.oh = s.rows; p.frames = s.frames; p.delta = delta;
     p.kch = 2 * (int)div_up((unsigned)(kw + FF_N - 1), 16);                 // K = kw + 31 rounded up to a multiple of 16 elements
-    p.tiles_x = (int)div_up((unsigned)p.ow, FF_N); p.tiles_y = (int)div_up((unsigned)p.oh, 128 * FF_MT);
+    p.tiles_x = (int)div_up((unsigned)p.ow, FF_N); p.tiles_y = (int)div_up((unsigned)p.oh, 128 * FF_WG);
     const long long nt = (long long)p.tiles_x * p.tiles_y * p.frames;
     if (nt > 0x7fffffff) return B200CV_NOT_IMPLEMENTED;
     p.ntiles = (int)nt;
-    const int ra = 128 * FF_MT + kh - 1;
+    const int ra = 128 * FF_WG + kh - 1;
     p.nbox = (ra + 255) / 256;
     p.box_h = (((ra + p.nbox - 1) / p.nbox) + 7) & ~7;
     p.ra_alloc = p.nbox * p.box_h;

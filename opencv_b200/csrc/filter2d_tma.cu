@@ -7,7 +7,7 @@
 // BORDER_CONSTANT; boundary CTAs patch the apron for the mirrored modes), 8-bit tiles are widened to float once per element
 // (PRMT into the mantissa of 2^23 + FADD, no I2F), each thread keeps an 8-output row segment in registers and walks the kernel rows
 // with 128-bit shared loads, and results leave as 8-byte (u8) or 2 x 16-byte (f32) stores.  The previous kernel spent its time in
-// per-element border arithmetic and scalar loads/stores: 0.41 ms for 3x3 on 16 4K frames against 0.04 ms of HBM time.
+// per-element border arithmetic and scalar loads/stores, far from the HBM time.
 #include <cstring>
 #include "common.cuh"
 #include "tma.cuh"

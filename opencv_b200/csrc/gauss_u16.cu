@@ -1,4 +1,4 @@
-// gauss_u16.cu -- cv::GaussianBlur for CV_16U images (SURVEY 8(a1): "u8 / u16: integer 8.8 / 16.16 fixed point, bit-exact").
+// gauss_u16.cu -- cv::GaussianBlur for CV_16U images ("u8 / u16: integer 8.8 / 16.16 fixed point, bit-exact").
 //
 // Reference: fixedSmoothInvoker<uint16_t, ufixedpoint32> (smooth.simd.hpp:1925-2197), taps getGaussianKernelFixedPoint_ED with 16 fractional
 // bits (smooth.dispatch.cpp:224-258), arithmetic fixedpoint.inl.hpp (ufixedpoint32 / ufixedpoint64):

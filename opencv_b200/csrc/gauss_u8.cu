@@ -282,8 +282,7 @@ int gauss_u8_fast(const Img& s, const Img& d, int cn, const int64_t* fx, int kw,
     for (int i = 0; i < kh; i++) sy += fy[i];
     if (sx > 256 || sy > 256) return B200CV_NOT_IMPLEMENTED;      // 16-bit row sums and an unsaturated result byte
     // GaussianBlur 3 x 3 / 5 x 5 with the binomial 8.8 taps (sigma = 0), one channel, 16-byte aligned rows of a multiple of 16 pixels: packed
-    // 16-bit adds, no multiplier, rows through a lane-private cp.async ring (gauss_u8_binomial.cu).  Measured on a B200, 16 4K frames: 0.0645 /
-    // 0.0741 ms (0.63 / 0.55 of the HBM roofline) against 0.074 / 0.087 (0.58 / 0.47) for the TMA tile kernel below, which keeps every other case
+    // 16-bit adds, no multiplier, rows through a lane-private cp.async ring (gauss_u8_binomial.cu).  The TMA tile kernel below keeps every other case
     // and is forced by B200CV_GAUSS_U8_PATH=tile (tests run both)
     if (sep_mode == 0 && !box) {
         const char* e = getenv("B200CV_GAUSS_U8_PATH");
@@ -305,9 +304,8 @@ int gauss_u8_fast(const Img& s, const Img& d, int cn, const int64_t* fx, int kw,
             p.kyw[o][g] = w;
         }
     // single channel, K <= 9, Gaussian / 8.8 sepFilter2D epilogues: the warp-streaming register kernel (gauss_u8_march.cu) exists as a second
-    // version; measured on a B200 (profiles/r02_notes.md) it executes fewer instructions (8.9 vs 12.1 per pixel at K = 3) but is 3-7 % SLOWER for
-    // GaussianBlur and 10-28 % slower in sepFilter2D's 8.8 mode (IDP on the half-rate pipe is the bound in both; its per-warp chunks give the
-    // memory system less in flight), so the tile kernel below stays the default; B200CV_GAUSS_U8_PATH=stream selects it (tests run both)
+    // version; it executes fewer instructions per pixel but gives the memory system less in flight (per-warp chunks), so the tile kernel
+    // below stays the default; B200CV_GAUSS_U8_PATH=stream selects it (tests run both)
     {
         const char* e = getenv("B200CV_GAUSS_U8_PATH");
         if (e && !strcmp(e, "stream") && cn == 1 && KB <= 9 && sep_mode <= 1) return gauss_u8_march(s, d, KB, tx, ty, border, st, sep_mode, even_limit);

@@ -7,7 +7,7 @@
 // (B + 128) >> 8, B <= 256 * 255 -- both fit 16 bits, rounding constant included.  So two pixels ride in one 32-bit register as 16-bit halves
 // and the whole filter is adds and shifts on the integer pipes, with no multiplier in the loop:
 //   IDP4A / IDP2A issue at half rate on the FMA-heavy pipe; the general tile kernel (gauss_u8.cu) spends ~3.5 of the ~11 issue slots per pixel that
-//   the HBM roofline leaves on them alone (12.1 thread-instructions per pixel at 3 x 3: 0.58 of the roofline, profiles/r02_notes.md section 2).
+//   the HBM roofline leaves on them alone, and is instruction-issue bound at 3 x 3.
 // A thread owns 16 adjacent columns (one 128-bit load per row) and walks down GB_SEG output rows: per word E / O = even / odd pixels as halves, the
 // shifted pairs by PRMT, row sums for the even and the odd pixels; the last K - 1 row sums stay in registers (ring resolved at compile time by
 // unrolling); column sums, rounding, one PRMT to bytes per word, one 128-bit store.  Rows outside the image are fetched from the reflected row
@@ -56,7 +56,7 @@ __device__ __forceinline__ void gb_cp4(void* smem, const void* g, int src_bytes)
 
 // A thread owns 16 adjacent columns and walks down GB_SEG rows.  Its rows arrive through a lane-private ring in shared memory filled by cp.async
 // (one 16-byte copy per row and lane = 512 contiguous bytes per warp and row, GB_DEPTH rows in flight, no registers held by loads in flight: with
-// loads into registers the kernel was latency bound -- 4-byte lanes 0.19 ms, 16-byte lanes 0.10 ms per 16 4K frames).  Nothing in the ring is shared
+// loads into registers the kernel was latency bound).  Nothing in the ring is shared
 // between lanes, so cp.async.wait_group is the only synchronisation.  The word left of the thread's first and right of its last word come from the
 // neighbouring lanes by shuffle; lanes 0 and 31 copy theirs; at the image edges they are built from the row's own bytes by the border rule.
 template <int K, bool FAST>

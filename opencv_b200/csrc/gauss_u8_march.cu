@@ -6,10 +6,9 @@
 // evaluator modules/imgproc/test/test_smooth_bitexact.cpp:40-53):
 //     dst = ((sum_j ky[j] * (sum_i kx[i] * src)) + 2^15) >> 16      8.8 taps, 16-bit row sums, bit for bit.
 //
-// History (profiles/r02_notes.md): v1 (gauss_u8.cu) = row pass -> shared memory -> barrier -> column pass on 4 x 4 items: 12.1 thread
-// instructions per pixel at K = 3, issue bound at 0.58 of the HBM roofline.  v2 = one CTA per 224 x 128 tile, registers only: 9.5
-// instructions per pixel but 0.62: a quarter of the warp cycles sat in the CTA barrier behind the tile's TMA load, and each warp filtered
-// K-1 rows twice.  v3 (this file):
+// History: v1 (gauss_u8.cu) = row pass -> shared memory -> barrier -> column pass on 4 x 4 items, instruction-issue bound.  v2 = one CTA
+// per 224 x 128 tile, registers only: fewer instructions per pixel, but the warps waited in the CTA barrier behind the tile's TMA load, and
+// each warp filtered K-1 rows twice.  v3 (this file):
 //   * worker = one warp.  It owns (frame, 224-column strip, segment of rows) and walks DOWN it in chunks of CH rows: lane 0 issues one
 //     3-D TMA box (256 x CH bytes) per chunk into one of the warp's two private buffers, one chunk ahead; completion on the warp's own
 //     mbarrier.  No CTA-wide barrier anywhere, no launch per tile: the grid is one wave of 4-warp CTAs, each warp loops over its items.
@@ -24,7 +23,7 @@
 //                   taps in bytes 2-3; the window rotates by loop unrolling (CH/2 is a multiple of K/2+1);
 //       epilogue    result byte = bits 16..23 (3 PRMT per 4 pixels), one 64-bit store per lane and row.
 // IDP runs on the half-rate FMA-heavy pipe: 3.5 / 5 / 6.5 / 8 IDP per pixel at K = 3 / 5 / 7 / 9 bound K = 7 and 9 below the HBM
-// roofline whatever else is done (DESIGN.md section 5).
+// roofline whatever else is done.
 #include <string.h>
 #include <algorithm>
 #include "common.cuh"

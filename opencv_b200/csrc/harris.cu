@@ -207,7 +207,7 @@ __global__ void __launch_bounds__(256) harris_kernel(Img src, Img dst, const __g
 
 // ---- second version for the common case (3-tap Sobel, block size 2 or 3): register marching, interior tiles only ------------------------------
 // The tile kernel above spends ~140 thread instructions per pixel on staging, three shared-memory passes and 4 BS^2 float -> double conversions
-// (profiles/r02_prof_harris_*.txt: issue-bound at 25 % occupancy).  Here a THREAD owns 4 adjacent output columns and walks down HF_SEG rows:
+// (issue-bound at 25 % occupancy).  Here a THREAD owns 4 adjacent output columns and walks down HF_SEG rows:
 // the 3-row windows of the two row-filtered derivative images, the current product row and the horizontal box sums of the previous BS - 1
 // product rows all live in registers (the row loop is unrolled by 6 = lcm(3, 2) so every ring index is a compile-time constant); a product is
 // converted to double once; no shared memory, no barrier; one 16-byte store per thread and row.  Arithmetic and operation order are the tile
@@ -487,8 +487,8 @@ constexpr int GC_R = 8;        // rows per tile of the candidate kernel (4 colum
 
 // Candidates = pixels that survive threshold(eig, max * quality, TOZERO) and equal the 3x3 maximum of the thresholded map (dilate + compare,
 // modules/imgproc/src/featureselect.cpp:127-166), 1-pixel frame excluded.  A thread walks down GC_R rows of 4 columns with the three window rows in
-// registers; the block reserves its output range with ONE atomic per 1024 x GC_R tile (a per-candidate atomic on the frame's counter serialises:
-// 10^6 candidates on a noisy 4K frame cost 0.16 ms per frame that way); the histogram of the response codes' top 12 bits (for the top-K
+// registers; the block reserves its output range with ONE atomic per 1024 x GC_R tile (a per-candidate atomic on the frame's counter serialises
+// on a noisy frame with many candidates); the histogram of the response codes' top 12 bits (for the top-K
 // preselection below) is kept in shared memory and flushed once per block.
 __global__ void __launch_bounds__(256) gftt_candidates_kernel(Img eig, const unsigned* maxord, double quality, CandKey* out, int cap, int* counts, unsigned* hist)
 {
@@ -654,7 +654,7 @@ extern "C" int b200cv_good_features_to_track(const b200cvMat* src, float* corner
     rc = corner_response(src, &eig, block_size, gradient_size, k, B200CV_BORDER_REFLECT_101, use_harris ? 0 : 1, stream);
     if (rc) { cleanup(); return rc; }
     Img e = make_img(&eig);
-    frame_max_kernel<<<dim3(std::min((unsigned)H, 148u * 8u), frames), 256, 0, st>>>(e, d_max);
+    frame_max_kernel<<<dim3(std::min((unsigned)H, (unsigned)num_sms() * 8u), frames), 256, 0, st>>>(e, d_max);
     count_launch();
     // top-K preselection (all frames, before the one synchronisation that brings the counts back)
     unsigned* d_hist = nullptr; int* d_thr = nullptr; int* d_topcnt = nullptr; CandKey* d_top = nullptr;
@@ -673,7 +673,7 @@ extern "C" int b200cv_good_features_to_track(const b200cvMat* src, float* corner
     }
     {
         const unsigned tiles = div_up(W, 1024) * div_up(H, GC_R);
-        gftt_candidates_kernel<<<dim3(std::min(tiles, 148u * 8u), frames), 256, 0, st>>>(e, d_max, quality_level, d_cand, cap, d_cnt, d_hist);
+        gftt_candidates_kernel<<<dim3(std::min(tiles, (unsigned)num_sms() * 8u), frames), 256, 0, st>>>(e, d_max, quality_level, d_cand, cap, d_cnt, d_hist);
         count_launch();
         TRY(cudaGetLastError());
     }

@@ -1,4 +1,4 @@
-// integral.cu -- cv::integral for 8UC1 images: sum (CV_32S) and, optionally, the sum of squares (CV_64F)  (SURVEY 8(f) rank 2).
+// integral.cu -- cv::integral for 8UC1 images: sum (CV_32S) and, optionally, the sum of squares (CV_64F) .
 //
 // Reference (sumpixels.dispatch.cpp:192-235, :415-451): sum is (H+1) x (W+1), first row and column zero,
 //     sum[y+1][x+1] = sum[y][x+1] + (src[y][0] + ... + src[y][x]);  int arithmetic (it wraps for images beyond 2^31 / 255 pixels, as the

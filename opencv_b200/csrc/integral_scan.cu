@@ -19,7 +19,7 @@ template <typename T, bool SQ> __device__ __forceinline__ T ig_val(uchar v)
 //          sum[y + 1][1 ..]; the same kernel zeroes column 0 and row 0
 // columns  one thread per column walks down the image adding in place, 8 rows of loads in flight; coalesced across the threads of a warp
 // Traffic: 1 byte read + 4 written (rows) + 4 read + 4 written (columns) = 13 bytes per pixel against 5 algorithmic; the first version moved
-// 1 + 4 + 1 + 4 + 4 + 4 + 4 = 22 and wrote its rows with uncoalesced 4-byte stores (0.53 TB/s algorithmic, profiles/r02_baseline_time_ops.txt).
+// 1 + 4 + 1 + 4 + 4 + 4 + 4 = 22 and wrote its rows with uncoalesced 4-byte stores.
 template <typename T> __device__ __forceinline__ T ig_shfl_up(T v, int d)
 {
     if constexpr (sizeof(T) == 8) {

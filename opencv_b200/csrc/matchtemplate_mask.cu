@@ -1,4 +1,4 @@
-// matchtemplate_mask.cu -- cv::matchTemplate with a mask (SURVEY 8(f) rank 4), one channel, 8-bit or float images / templates, 8-bit (binarised)
+// matchtemplate_mask.cu -- cv::matchTemplate with a mask, one channel, 8-bit or float images / templates, 8-bit (binarised)
 // or float (weight) masks, all six methods.
 //
 // Reference (matchTemplateMask, templmatch.cpp:762-905): everything becomes float, then up to four cross-correlations through the block DFT:

@@ -1,4 +1,4 @@
-// matchtemplate_tc.cu -- the matchTemplate correlation numerator on 5th-generation tensor cores (tcgen05, kind::i8).
+// matchtemplate_tc.cu -- the matchTemplate correlation numerator on Hopper tensor cores (wgmma, u8 x u8 -> s32).
 //
 //   R(y, x) = sum_{v<h} sum_{u<w} T(v,u) * I(y+v, x+u)          8-bit image and template, exact 32-bit integer result
 //
@@ -8,10 +8,10 @@
 // A_v is a plain 128-byte-wide box of image rows -- NO im2col is materialised: the CTA stages rows y0 .. y0+M+h-2 once
 // (TMA, 16-byte-column boxes = the canonical K-major no-swizzle core-matrix layout) and the A descriptor of step v simply
 // starts v rows (v*16 bytes) further down.  B_v (8 KB) is pre-expanded once per call into global memory in the same layout
-// and streamed through a 4-stage cp.async.bulk ring.  One elected thread issues tcgen05.mma (M=128, N=64, K=32, u8 x u8 ->
-// s32, accumulators in TMEM, two M-tiles per CTA share every B_v), tcgen05.commit frees ring slots and publishes the
-// accumulator; all four warps read it back with tcgen05.ld and store float(R).  Half of B is zeros (2.1x redundant MACs),
-// the price of a well-shaped MMA (SURVEY 7.2); the result is exact because products <= 65025 and sums < 2^31.
+// and streamed through a 4-stage cp.async.bulk ring by a producer warp.  Two consumer warpgroups each own 128 output rows
+// (two wgmma m64n64k32 slabs sharing every B_v, accumulators in registers) and store float(R) from their registers.  Half of B
+// is zeros (2.1x redundant MACs), the price of a well-shaped MMA; the result is exact because products <= 65025
+// and sums < 2^31.
 //
 //
 // (8-bit filter2D with >= 11x11 taps uses the same Toeplitz formulation in a persistent kernel: filter2d_tc.cu.)
@@ -19,6 +19,7 @@
 // Reference: crossCorr, modules/imgproc/src/templmatch.cpp:566-760 (block DFT in float on one thread).
 #include "common.cuh"
 #include "tma.cuh"
+#include "wgmma.cuh"
 #include <cmath>
 #include <vector>
 
@@ -26,7 +27,8 @@ namespace b200cv {
 
 constexpr int TC_N = 64;          // outputs per x-tile (MMA N)
 constexpr int TC_K = 128;         // K per template row: w + N - 1 <= 128
-constexpr int TC_MT = 2;          // M-tiles (of 128 rows) per CTA
+constexpr int TC_WG = 2;          // consumer warpgroups per CTA, 128 output rows each
+constexpr int TC_THREADS = 128 * TC_WG + 32;   // + one producer warp
 constexpr int TC_NS = 4;          // B ring stages
 constexpr int TC_BBYTES = TC_N * TC_K;   // 8192
 
@@ -74,152 +76,94 @@ __global__ void __launch_bounds__(128) pad_u8_kernel(Img src, Img dst, int ax, i
     *(uint4*)(dst.row<uchar>(f, y) + x16) = make_uint4(o[0], o[1], o[2], o[3]);
 }
 
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes)
-{
-    // K-major, no swizzle: start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | version=1 [46,48) | layout_type=0 [61,64)
-    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) | (1ull << 46);
-}
-
-__device__ __forceinline__ void umma_i8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}"
-                 ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// one lane of a converged warp: the issuer warp runs its loop warp-uniformly and elects the issuing thread, so the descriptors stay in
-// uniform registers (issued from inside `if (lane == 0)` every operand went through an R2UR waterfall: ~15 instructions per MMA)
-__device__ __forceinline__ bool umma_elect_one()
-{
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void bulk_load(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar)
-{
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r)
-{
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]),
-          "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]),
-          "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr) : "memory");
-}
-
 struct TCParams {
     int h, ra_alloc, box_h, nbox;       // template rows; staged image rows (allocated), rows per TMA box, boxes per column chunk
     int ow, oh;
     int kch;                            // K per template row = 32 * kch (w + N - 1 <= 32 * kch)
 };
 
-__global__ void __launch_bounds__(128) ccorr_u8_tc_kernel(const __grid_constant__ CUtensorMap tmap, const unsigned char* __restrict__ bglob, Img res, TCParams p)
+__global__ void __launch_bounds__(TC_THREADS) ccorr_u8_tc_kernel(const __grid_constant__ CUtensorMap tmap, const unsigned char* __restrict__ bglob, Img res, TCParams p)
 {
     constexpr int NN = TC_N;                                           // MMA N
-    constexpr int TCOLS = TC_MT * NN <= 128 ? 128 : TC_MT * NN <= 256 ? 256 : 512;   // TMEM columns (power of two)
     extern __shared__ __align__(128) unsigned char smem[];
     const int nchunk = 2 * p.kch;                                      // 16-byte K chunks per row
     const uint32_t bbytes = (uint32_t)nchunk * NN * 16;                // one B slab
     unsigned char* sA = smem;                                          // nchunk x ra_alloc rows x 16 B
     unsigned char* sB = smem + (size_t)nchunk * p.ra_alloc * 16;       // TC_NS slabs
-    __shared__ __align__(8) uint64_t full[TC_NS], empty[TC_NS], a_full, acc_full;
-    __shared__ uint32_t s_tmem;
+    __shared__ __align__(8) uint64_t full[TC_NS], empty[TC_NS], a_full;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int f = blockIdx.z, x0 = blockIdx.x * TC_N, y0 = blockIdx.y * (128 * TC_MT);
+    const int f = blockIdx.z, x0 = blockIdx.x * TC_N, y0 = blockIdx.y * (128 * TC_WG);
     const uint32_t lbo_a = (uint32_t)p.ra_alloc * 16u;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < TC_NS; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        mbar_init(&a_full, 1); mbar_init(&acc_full, 1);
+        for (int s = 0; s < TC_NS; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 4 * TC_WG); }
+        mbar_init(&a_full, 1);
         fence_barrier_init();
     }
-    if (warp == 0) {   // TMEM: TC_MT x NN columns of 32-bit accumulators
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)), "r"(TCOLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = s_tmem;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 4 * TC_WG) {
         // ---- producer: image rows once, then the Toeplitz operand of every template row through the ring ----
-        mbar_arrive_expect_tx(&a_full, (uint32_t)p.ra_alloc * 16u * nchunk);
-        for (int c = 0; c < nchunk; c++)
-            for (int b = 0; b < p.nbox; b++)
-                tma_load_3d(sA + (size_t)c * lbo_a + (size_t)b * p.box_h * 16, &tmap, x0 + 16 * c, y0 + b * p.box_h, f, &a_full);
-        for (int v = 0; v < p.h; v++) {
-            const int s = v % TC_NS;
-            mbar_wait(&empty[s], ((v / TC_NS) & 1) ^ 1);
-            mbar_arrive_expect_tx(&full[s], bbytes);
-            bulk_load(sB + (size_t)s * bbytes, bglob + (size_t)v * bbytes, bbytes, &full[s]);
-        }
-    } else if (warp == 1) {
-        // ---- MMA issuer: the whole warp runs the loop (uniform values), one elected lane issues ----
-        // instruction descriptor: D = S32 (2<<4), A = B = unsigned 8 bit (0 at [7,10) and [10,13)),
-        // K-major both, N>>3 at [17,23), M>>4 at [24,29)
-        const uint32_t idesc = (2u << 4) | ((uint32_t)(NN >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-        mbar_wait(&a_full, 0);
-        tc_fence_after();
-        // descriptors (K-major, no swizzle): low word = start >> 4 [0,14) | LBO >> 4 [16,30); high word = SBO >> 4 | version 1 at bit 14
-        const uint32_t hi = (128u >> 4) | (1u << 14);
-        const uint32_t a_lo0 = ((smem_u32(sA) & 0x3FFFFu) >> 4) | ((lbo_a >> 4) << 16);
-        const uint32_t b_lo0 = ((smem_u32(sB) & 0x3FFFFu) >> 4) | (((uint32_t)(NN * 16) >> 4) << 16);
-        const uint32_t a_ks = (2u * lbo_a) >> 4;
-        for (int v = 0; v < p.h; v++) {
-            const int s = v % TC_NS;
-            mbar_wait(&full[s], (v / TC_NS) & 1);
-            tc_fence_after();
-            if (umma_elect_one()) {
-#pragma unroll
-                for (int mt = 0; mt < TC_MT; mt++)
-#pragma unroll
-                    for (int ks = 0; ks < TC_K / 32; ks++) {
-                        if (ks < p.kch) {
-                            const uint64_t ad = ((uint64_t)hi << 32) | (a_lo0 + (uint32_t)ks * a_ks + (uint32_t)(mt * 128 + v));
-                            const uint64_t bd = ((uint64_t)hi << 32) | (b_lo0 + (((uint32_t)s * bbytes) >> 4) + (uint32_t)ks * ((2u * NN * 16) >> 4));
-                            umma_i8(tmem + mt * NN, ad, bd, idesc, (v | ks) != 0);
-                        }
-                    }
-                umma_commit(&empty[s]);
+        if (lane == 0) {
+            mbar_arrive_expect_tx(&a_full, (uint32_t)p.ra_alloc * 16u * nchunk);
+            for (int c = 0; c < nchunk; c++)
+                for (int b = 0; b < p.nbox; b++)
+                    tma_load_3d(sA + (size_t)c * lbo_a + (size_t)b * p.box_h * 16, &tmap, x0 + 16 * c, y0 + b * p.box_h, f, &a_full);
+            for (int v = 0; v < p.h; v++) {
+                const int s = v % TC_NS;
+                mbar_wait(&empty[s], ((v / TC_NS) & 1) ^ 1);
+                mbar_arrive_expect_tx(&full[s], bbytes);
+                wg_bulk_load(sB + (size_t)s * bbytes, bglob + (size_t)v * bbytes, bbytes, &full[s]);
             }
-            __syncwarp();
         }
-        if (umma_elect_one()) umma_commit(&acc_full);
+        return;
     }
-    // ---- epilogue: all four warps; warp w owns TMEM lanes (= accumulator rows) 32w .. 32w+31 ----
-    __syncwarp();
-    mbar_wait(&acc_full, 0);
-    tc_fence_after();
-#pragma unroll 1
-    for (int mt = 0; mt < TC_MT; mt++) {
-        const int gy = y0 + mt * 128 + warp * 32 + lane;
-        const uint32_t trow = tmem + ((uint32_t)(warp * 32) << 16) + mt * NN;
-#pragma unroll 1
-        for (int half = 0; half < 2; half++) {
-            uint32_t r[32];
-            tmem_ld32(trow + half * 32, r);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            float* rp = gy < p.oh ? res.row<float>(f, gy) + x0 : nullptr;
-            if (rp) {
+
+    // ---- consumers: warpgroup wg owns accumulator rows 128 wg .. 128 wg + 127 as two 64-row slabs ----
+    const int wg = warp >> 2, wl = warp & 3;
+    uint32_t acc[2][NN / 2];
 #pragma unroll
-                for (int j = 0; j < 32; j++) {
-                    int gx = x0 + half * 32 + j;
-                    if (gx < p.ow) rp[half * 32 + j] = (float)(int)r[j];
+    for (int m = 0; m < 2; m++)
+#pragma unroll
+        for (int r = 0; r < NN / 2; r++) acc[m][r] = 0;
+    mbar_wait(&a_full, 0);
+    wg_fence();
+    const uint32_t a0 = smem_u32(sA) + (uint32_t)(wg * 128) * 16u, b0 = smem_u32(sB);
+    int prev = -1;
+    for (int v = 0; v < p.h; v++) {
+        const int s = v % TC_NS;
+        mbar_wait(&full[s], (v / TC_NS) & 1);
+#pragma unroll
+        for (int ks = 0; ks < TC_K / 32; ks++) {
+            const uint64_t bd = wg_desc(b0 + (uint32_t)s * bbytes + (uint32_t)ks * (2 * NN * 16), NN * 16, 128);
+#pragma unroll
+            for (int m = 0; m < 2; m++)    // the A operand of template row v starts v image rows (v x 16 bytes) further down
+                wgmma_u8u8_n64(acc[m], wg_desc(a0 + (uint32_t)ks * 2u * lbo_a + (uint32_t)(m * 64 + v) * 16u, lbo_a, 128), bd);
+        }
+        wg_commit();
+        wg_wait<1>();                      // the previous row's MMAs are done: its ring slot may be refilled
+        wg_mbar_arrive_if(&empty[prev < 0 ? 0 : prev], lane == 0 && prev >= 0);
+        prev = s;
+    }
+    wg_wait<0>();
+    wg_fence_operand(acc[0]);
+    wg_fence_operand(acc[1]);
+    // ---- epilogue straight from the accumulator registers ----
+#pragma unroll
+    for (int m = 0; m < 2; m++)
+#pragma unroll
+        for (int i = 0; i < 2; i++) {
+            const int gy = y0 + wg * 128 + m * 64 + wl * 16 + (lane >> 2) + 8 * i;
+            if (gy >= p.oh) continue;
+            float* rp = res.row<float>(f, gy);
+#pragma unroll
+            for (int j = 0; j < NN / 8; j++)
+#pragma unroll
+                for (int c = 0; c < 2; c++) {
+                    const int gx = x0 + 8 * j + 2 * (lane & 3) + c;
+                    if (gx < p.ow) rp[gx] = (float)(int)acc[m][4 * j + 2 * i + c];
                 }
-            }
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(TCOLS) : "memory");
 }
 
 // returns B200CV_NOT_IMPLEMENTED when the tensor-core path does not apply (caller uses the IDP4A kernel)
@@ -229,7 +173,7 @@ int ccorr_u8_tensor(const Img& im, const Img& tp, const Img& rs, int w, int h, c
     const int ow = im.cols - w + 1, oh = im.rows - h + 1;
     TCParams p;
     p.h = h; p.ow = ow; p.oh = oh; p.kch = TC_K / 32;
-    int ra = 128 * TC_MT + h - 1;
+    int ra = 128 * TC_WG + h - 1;
     p.nbox = (ra + 255) / 256;
     p.box_h = (((ra + p.nbox - 1) / p.nbox) + 7) & ~7;
     p.ra_alloc = p.nbox * p.box_h;
@@ -244,8 +188,8 @@ int ccorr_u8_tensor(const Img& im, const Img& tp, const Img& rs, int w, int h, c
     CUtensorMap tm;
     int rc = make_tensor_map_3d(&tm, im.data, 1, im.cols, im.rows, im.frames, im.step, im.fstep, 16, p.box_h);
     if (rc) { cudaFreeAsync(bglob, st); return rc; }
-    dim3 grid(div_up((unsigned)ow, TC_N), div_up((unsigned)oh, 128 * TC_MT), (unsigned)im.frames);
-    ccorr_u8_tc_kernel<<<grid, 128, smem, st>>>(tm, bglob, rs, p);
+    dim3 grid(div_up((unsigned)ow, TC_N), div_up((unsigned)oh, 128 * TC_WG), (unsigned)im.frames);
+    ccorr_u8_tc_kernel<<<grid, TC_THREADS, smem, st>>>(tm, bglob, rs, p);
     cudaError_t e = cudaGetLastError();
     cudaFreeAsync(bglob, st);
     count_launch();

@@ -1,4 +1,4 @@
-// pyramid.cu -- cv::pyrDown / cv::pyrUp (SURVEY 8(f) "next": the image-pyramid callers of the blur path).
+// pyramid.cu -- cv::pyrDown / cv::pyrUp (the image-pyramid callers of the blur path).
 //
 // pyrDown (pyramids.cpp:884-1039): 5-tap [1 4 6 4 1] rows into an intermediate at every second column, the same taps over every
 // second row, then a 1/256 cast; borders through cv::borderInterpolate on the SOURCE coordinates (any mode but CONSTANT).

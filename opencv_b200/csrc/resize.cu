@@ -145,7 +145,7 @@ __device__ __forceinline__ int rs_dp2a(int a, unsigned b, int c)
 constexpr int RS_ROWS = 8;   // destination rows per thread
 // (Two shared-memory tiled variants were measured and dropped: staging the footprint and filtering every source row once, with
 //  the intermediate rows in shared memory or in a per-thread register ring, ran at 12-24 resident warps per SM and were latency
-//  bound -- 0.52-1.9 ms against 0.30-1.3 ms for the kernels below on the 8K->5K and 4K->8K cases, profiles/r01_notes.md.)
+//  bound, slower than the kernels below on the 8K->5K and 4K->8K cases.)
 
 // ---- LINEAR ----------------------------------------------------------------------------------------------------------
 template <typename T, int CN>
@@ -417,8 +417,8 @@ static int resize_impl(const b200cvMat* src, const b200cvMat* dst, int interpola
         dim3 g4(div_up(div_up((unsigned)p.dw, 4), 128), (unsigned)p.dh, (unsigned)s.frames);
         int vec_ok = (((uintptr_t)d.data | d.step | d.fstep) & 3) == 0 && (pix % 4 != 0 || (((uintptr_t)s.data | s.step | s.fstep) & 3) == 0);
         const char* nn_env = getenv("B200CV_RESIZE_NN_PATH");              // "v1": the per-pixel kernel always; "walk": the walking kernel whenever it applies
-        // only when rows repeat (enlarging in y): measured 4K -> 8K 8UC3 0.164 -> 0.137 ms per 4 frames, but 8K -> 4K 0.072 -> 0.085 (the per-pixel
-        // kernel has 32x the threads in flight for the same gathers)
+        // only when rows repeat (enlarging in y): there the walking kernel reuses each gathered row; when shrinking, the per-pixel kernel
+        // has 32x the threads in flight for the same gathers
         const bool walk = (nn_env && !strcmp(nn_env, "walk")) || (p.dh > p.sh && !(nn_env && !strcmp(nn_env, "v1")));
         if (walk && depth == B200CV_8U && (pix == 1 || pix == 3 || pix == 4) && (((uintptr_t)d.data | d.step | d.fstep) & 3) == 0) {
             dim3 gw(div_up(div_up((unsigned)p.dw, 4), 128), div_up((unsigned)p.dh, NN_ROWS), (unsigned)s.frames);

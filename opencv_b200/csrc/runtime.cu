@@ -32,9 +32,9 @@ void count_launch(int n) { g_launches.fetch_add((unsigned long long)n, std::memo
 int num_sms()
 {
     int dev = 0, n = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
     int& slot = g_num_sms[dev & 63];
-    if (slot == 0) slot = (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0) ? n : 148;
+    if (slot == 0) slot = (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0) ? n : 132;
     return slot;
 }
 
@@ -48,8 +48,8 @@ int check_mat(const b200cvMat* m, const char* name)
 }
 
 // Scratch buffers (padded images, coefficient tables, candidate lists) are stream-ordered allocations.  By default the pool hands
-// unused memory back to the OS at every synchronisation, so the next call pays a fresh allocation (measured: 2 ms for a 256 KB table
-// after a device synchronise; the host path synchronises after every op).  Keep the memory in the pool.
+// unused memory back to the OS at every synchronisation, so the next call pays a fresh allocation (the host path
+// synchronises after every op).  Keep the memory in the pool.
 void configure_mem_pool()
 {
     int dev = 0;
@@ -72,7 +72,7 @@ using namespace b200cv;
 extern "C" {
 
 const char* b200cv_last_error(void) { return g_err; }
-const char* b200cv_version(void) { return "b200cv 0.1 (sm_100a)"; }
+const char* b200cv_version(void) { return "b200cv 0.1 (sm_90a)"; }
 unsigned long long b200cv_launch_count(void) { return g_launches.load(); }
 
 int b200cv_device_count(void)
@@ -96,8 +96,8 @@ int b200cv_init(int device)
     B200_CUDA(cudaSetDevice(device));
     cudaDeviceProp p;
     B200_CUDA(cudaGetDeviceProperties(&p, device));
-    if (p.major != 10) {
-        set_error("device %d is sm_%d%d; this library contains sm_100a code only", device, p.major, p.minor);
+    if (p.major != 9 || p.minor != 0) {
+        set_error("device %d is sm_%d%d; this library contains sm_90a code only", device, p.major, p.minor);
         return B200CV_ERR_NO_DEVICE;
     }
     g_num_sms[device & 63] = p.multiProcessorCount;

@@ -10,7 +10,7 @@
 // Same arithmetic as sep_fast_kernel<.,.,M_FLOAT,KB> in sepfilter.cu -- only the data movement differs: ONE thread issues a 3-D cp.async.bulk.tensor box load of the
 // (192+2r) x (32+2r) float tile into shared memory and the CTA waits on an mbarrier, so the loads of one CTA overlap the
 // arithmetic of the other CTAs resident on the SM instead of stalling every thread on its own LDG (the generic kernel was
-// long-scoreboard bound: ncu profiles/r01_prof1_summary.txt).  TMA zero-fills outside the image (= BORDER_CONSTANT); for
+// long-scoreboard bound).  TMA zero-fills outside the image (= BORDER_CONSTANT); for
 // REPLICATE / REFLECT / REFLECT_101 only boundary CTAs patch their apron from the mirrored in-tile cells.
 #include <cstdlib>
 #include <cstring>
@@ -33,7 +33,7 @@ struct SF32Params {
 };
 
 // ---- up to 11 taps: the plain tile kernel (one 192 x 32 tile per CTA, 3 CTAs per SM at 80 registers) -- the walking kernel below carries
-//      state that does not fit that register budget (its tile form ran 8-15 % slower at 3 and 9 taps on a B200) ----
+//      state that does not fit that register budget (its tile form is slower at 3 and 9 taps) ----
 template <int KB, typename ST, typename DT>
 __global__ void __launch_bounds__(256, 3) sep_f32_tile_kernel(const __grid_constant__ CUtensorMap tmap, Img dst, const __grid_constant__ SF32Params p)
 {
@@ -233,7 +233,7 @@ static int launch_sf32_tile(const CUtensorMap& tm, const Img& d, const SF32Param
 // Kernels of 13 taps and more WALK DOWN a column strip (p.nch chunks of SF_TH output rows per CTA): the SF_TH + KB - 1 row-filtered rows behind
 // a chunk stay in shared memory, the last KB - 1 of them move to the top for the next chunk (a 20-word copy per thread), and every chunk after
 // the first stages and row-filters only its SF_TH new source rows -- the plain tile kernel filtered SF_TH + KB - 1 rows for SF_TH outputs
-// (1.9x the row-pass work at 27 taps: profiles/r02_prof_sift_sep_f32_before.txt, FFMA 63 per pixel).  The next chunk's TMA load is issued
+// (1.9x the row-pass work at 27 taps).  The next chunk's TMA load is issued
 // right after the row pass and lands during the column pass.  Rows above / below the image (mirroring borders): the row filter commutes
 // with the vertical mirror, so those filtered rows are copies of the mirrored rows' filtered rows.
 template <int KB, typename ST, typename DT>

@@ -70,7 +70,7 @@ __global__ void __launch_bounds__(256) sift_upsample2x_kernel(Img src, Img dst)
 // index arithmetic: min(floor(x * (1 / (dw / sw))), sw - 1) in double), then layer after layer the separable Gaussian in the operation order
 // of the library's float filter kernels (rows: fma in tap order from 0; columns: fma(ky[c], S[c], 0) then fma(ky[c+k], S[c+k] + S[c-k], .),
 // BORDER_REFLECT_101 by index), each DoG level with the blur that writes its minuend.  As separate launches these ~6 x 4 tiny dependent
-// kernels took 0.5 ms of a 5.4 ms pyramid batch (profiles/r02_launches_bench_c5.csv): a chain of launches, each far below one wave.
+// kernels are a chain of launches, each far below one wave.
 constexpr int SS_CAP = 3072;          // floats per level buffer
 constexpr int SS_MAXO = 8, SS_MAXL = 10, SS_MAXK = 33;
 struct SiftSmallParams {

@@ -1,4 +1,4 @@
-// sift_detect.cu -- the SIFT front end after the pyramid (SURVEY 8(f) rank 1): scale-space extrema, sub-pixel refinement, orientation
+// sift_detect.cu -- the SIFT front end after the pyramid: scale-space extrema, sub-pixel refinement, orientation
 // assignment and the 128-element descriptors, consuming the packed Gaussian / DoG pyramids that b200cv_sift_pyramid leaves in HBM.
 //
 // Reference: findScaleSpaceExtrema (sift.dispatch.cpp:368-402; sift.simd.hpp:400-681), adjustLocalExtrema (:291-397), calcOrientationHist

@@ -1,4 +1,4 @@
-// tma.cuh -- Tensor Memory Accelerator plumbing (sm_100a): tensor-map creation on the host (through the driver entry point,
+// tma.cuh -- Tensor Memory Accelerator plumbing (sm_90a): tensor-map creation on the host (through the driver entry point,
 // no link-time dependency on libcuda) and the mbarrier / cp.async.bulk.tensor PTX wrappers used by the tile kernels.
 #pragma once
 #include <cuda.h>

@@ -455,8 +455,8 @@ __global__ void __launch_bounds__(256) warp_tile_kernel(Img src, Img dst, const 
 }
 
 // ---- 8-bit LINEAR / CUBIC, second version of the tiled kernel -------------------------------------------------------------------------------
-// Same staging and the same sampling arithmetic as warp_tile_kernel; what changes is how the work is cut (profiles/r02_prof_c3_geom: the first
-// version executed 203 (LINEAR) to 345 (CUBIC, projective) thread instructions per pixel at 85 % issue utilisation, most of them not sampling):
+// Same staging and the same sampling arithmetic as warp_tile_kernel; what changes is how the work is cut (the first
+// version was instruction-issue bound, most of its instructions not sampling):
 //   * tile 128 x 32 instead of 64 x 16: the per-thread fixed costs (corner coordinates, tables, staged-row pointers and border tests) are
 //     spread over 16 pixels per thread instead of 4; the footprint of an 8UC3 tile is still only ~25 KB
 //   * a thread produces 4 consecutive pixels of a row: their bytes leave as CN aligned 32-bit stores (12 bytes of an 8UC3 row per thread, a
@@ -650,8 +650,7 @@ __global__ void __launch_bounds__(256) warp_tile4_kernel(Img src, Img dst, const
 }
 
 // ---- NEAREST, 8-bit: the coordinate tables of warp_tile4_kernel without the staging pass ---------------------------------------------------
-// The direct kernel evaluates the fp64 coordinate pipeline per pixel (96 thread instructions per pixel for an affine map, 174 for a projective
-// one: profiles/r02_prof_c3_geometry_before_*): here the affine adelta / bdelta / X0 / Y0 tables and the projective per-(row, column block)
+// The direct kernel evaluates the fp64 coordinate pipeline per pixel per pixel: here the affine adelta / bdelta / X0 / Y0 tables and the projective per-(row, column block)
 // terms are built once per 128 x 32 tile, a thread gathers 4 consecutive pixels and stores them as CN 32-bit words.
 template <int CN>
 __global__ void __launch_bounds__(256) warp_nn4_kernel(Img src, Img dst, const __grid_constant__ WarpParams p)

@@ -1,7 +1,7 @@
 """opencv_b200.hal -- the HOST-memory face: numpy arrays (cv::Mat layout) in, numpy arrays out.
 
 Each function is the cv2-named call over host memory; it goes through the batched host C ABI
-(b200cv_host_*, include/b200cv_hal.h): frames are uploaded, processed by the same sm_100a kernels and
+(b200cv_host_*, include/b200cv_hal.h): frames are uploaded, processed by the same sm_90a kernels and
 downloaded through a 3-stream pipeline.  Arrays: (H,W), (H,W,C) or a batch (N,H,W,C).
 `pinned_empty` allocates page-locked numpy arrays (b200cv_host_alloc) for full PCIe speed.
 """

@@ -354,7 +354,7 @@ API int ref_good_features_to_track(const void* src, size_t sstep, int w, int h, 
 
 // ---- the whole SIFT front end (detectAndCompute, sift.dispatch.cpp:501-580): keypoints + descriptors of the unmodified reference.
 // kp: 6 floats per keypoint (x, y, size, angle, response, octave as int bits), desc: 128 floats per keypoint; at most max_kp are written,
-// *n receives the number found.  The oracle for SURVEY 8(f) rank 1 (scale-space extrema, orientation, descriptors).
+// *n receives the number found.  The oracle for the SIFT front end (scale-space extrema, orientation, descriptors).
 API int ref_sift_detect_and_compute(const void* gray, size_t step, int w, int h, int nfeatures, int nOctaveLayers, double contrastThreshold,
                                     double edgeThreshold, double sigma, int precise_upscale, const void* mask, size_t mask_step, int max_kp, float* kp,
                                     float* desc, int* n)

@@ -1,8 +1,8 @@
 // The cv::-typed face (opencv_b200/host/b200cv_opencv.hpp) compiled against the REAL OpenCV headers of the reference
 // (-I/root/reference/modules/{core,imgproc}/include) and linked with the reference itself (oracle/_ref/libocvref.so = core + imgproc, no CUDA):
-// cv::InputArray kinds MAT, CUDA_GPU_MAT, CUDA_HOST_MEM (mat.hpp:163-188) reach the sm_100a kernels, cv::cuda::Filter usage as in
+// cv::InputArray kinds MAT, CUDA_GPU_MAT, CUDA_HOST_MEM (mat.hpp:163-188) reach the sm_90a kernels, cv::cuda::Filter usage as in
 // samples/cpp/tutorial_code/gpu/gpu-basics-similarity/gpu-basics-similarity.cpp:392-404, results checked against cv:: on the CPU.
-// Built here (tests/cpp/build_cv_surface.py; /root/reference is absent on the GPU box), run by tests/test_gpu_hal.py.  Exit code 0 = all checks passed.
+// Built into oracle/_ref/ by oracle/build_cv_surface.py where the reference's sources are, run by tests/test_gpu_hal.py.  Exit code 0 = all checks passed.
 #include <cstdio>
 #include <opencv2/core.hpp>
 #include <opencv2/imgproc.hpp>

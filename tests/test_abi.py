@@ -63,14 +63,12 @@ def test_cpp_host_mirror_compiles_against_the_c_abi():
 
 
 def test_cv_typed_surface_compiles_against_the_reference_headers():
-    """b200cv_opencv.hpp (cv::InputArray / OutputArray / cv::cuda::GpuMat / HostMem) builds against /root/reference's headers and links with
+    """b200cv_opencv.hpp (cv::InputArray / OutputArray / cv::cuda::GpuMat / HostMem) builds against the reference's headers and links with
     the reference's core + imgproc; without a device the binary fails loudly"""
     import subprocess
-    import sys
-    if not os.path.isdir("/root/reference/modules/core/include") or not os.path.exists(os.path.join(ROOT, "oracle", "_ref", "libocvref.so")):
-        pytest.skip("needs /root/reference and oracle/_ref")
-    sys.path.insert(0, os.path.join(ROOT, "tests", "cpp"))
-    import build_cv_surface
+    from oracle import build_cv_surface
+    if not os.path.isdir(os.path.join(build_cv_surface.REF, "modules", "core", "include")) or not os.path.exists(os.path.join(ROOT, "oracle", "_ref", "libocvref.so")):
+        pytest.skip("needs the reference's sources and oracle/_ref")
     exe = build_cv_surface.build()
     assert exe and os.path.exists(exe)
     import torch

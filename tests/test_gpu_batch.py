@@ -18,7 +18,7 @@ pytestmark = pytest.mark.gpu
 def driver(request, cvb):
     n = C.lib().b200cv_device_count()
     if request.param == "all" and n < 2:
-        pytest.skip("one GPU visible: the multi-device driver needs gpurun --gpus N")
+        pytest.skip("one GPU visible: the multi-device driver needs two or more")
     d = BatchDriver([0] if request.param == "one" else None)
     yield d
     d.close()

@@ -1,6 +1,6 @@
 """GPU parity: cv::cvtColor for the Bayer mosaics (BG / GB / RG / GR -> BGR, BGRA; bilinear and edge-aware), 8- and 16-bit: BIT-EXACT.
 
-First ran green on a B200 in round 1 (GPUTEST_r01.json); a failure here fails the suite."""
+A failure here fails the suite."""
 import numpy as np
 import pytest
 

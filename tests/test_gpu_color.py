@@ -71,6 +71,6 @@ def test_unaligned_rows(cvb, oracle, rng):
 
 @pytest.mark.parametrize("code,dcn", [(C.COLOR_BGR2GRAY, 1), (C.COLOR_BGR2YUV, 3), (C.COLOR_BGR2HSV, 3), (C.COLOR_YUV2BGR, 3), (C.COLOR_HSV2BGR, 3)])
 def test_cvt_8k(cvb, ref, rng, code, dcn):
-    """BASELINE config C3 (cvtColor leg) at full 7680x4320 size against the real reference"""
+    """bench.py workload c3 (cvtColor leg) at full 7680x4320 size against the real reference"""
     img = rand_u8(rng, 4320, 7680, 3)
     assert_exact(cpu(cvb.cvtColor(gpu(img), code, dcn)), ref.cvtColor(img, code, dcn), "8K code=%d" % code)

@@ -70,7 +70,7 @@ def test_match_template_f32(cvb, oracle, rng, method):
 
 
 def test_match_template_4k(cvb, ref, rng):
-    """BASELINE config C4: TM_CCORR_NORMED, 3840x2160 8UC1 frame vs a 64x64 crop at (1000,700)"""
+    """bench.py workload c4: TM_CCORR_NORMED, 3840x2160 8UC1 frame vs a 64x64 crop at (1000,700)"""
     img = rand_u8(rng, 2160, 3840)
     templ = img[700:764, 1000:1064].copy()
     want = ref.matchTemplate(img, templ, C.TM_CCORR_NORMED)
@@ -92,7 +92,7 @@ def test_corner_harris(cvb, oracle, rng, bs, ks, border):
 
 
 def test_corner_harris_4k(cvb, ref, rng):
-    """BASELINE config C4: cornerHarris(blockSize=2, ksize=3, k=0.04) on 3840x2160 8UC1"""
+    """bench.py workload c4: cornerHarris(blockSize=2, ksize=3, k=0.04) on 3840x2160 8UC1"""
     img = smooth_img(rng, 2160, 3840)
     want = ref.cornerHarris(img, 2, 3, 0.04)
     got = cpu(cvb.cornerHarris(gpu(img), 2, 3, 0.04))
@@ -115,7 +115,7 @@ def test_good_features(cvb, oracle, rng, harris, mind):
 
 
 def test_good_features_4k(cvb, ref, rng):
-    """BASELINE config C4: goodFeaturesToTrack(1000, 0.01, 10, blockSize 3, gradientSize 3, Harris k=0.04) on 4K"""
+    """bench.py workload c4: goodFeaturesToTrack(1000, 0.01, 10, blockSize 3, gradientSize 3, Harris k=0.04) on 4K"""
     img = smooth_img(rng, 2160, 3840)
     want, wq = ref.goodFeaturesToTrack(img, 1000, 0.01, 10, 3, 3, True, 0.04)
     got, gq = cvb.goodFeaturesToTrack(gpu(img), 1000, 0.01, 10, 3, 3, True, 0.04, with_quality=True)
@@ -184,7 +184,7 @@ def test_sift_pyramid_batch_1080p(cvb, ref, rng):
 
 
 def test_sift_pyramid_4k(cvb, ref, rng):
-    """BASELINE config C5 frame size: the whole Gaussian + DoG pyramid of one 3840x2160 8UC1 frame against the reference's
+    """bench.py workload c5 frame size: the whole Gaussian + DoG pyramid of one 3840x2160 8UC1 frame against the reference's
     buildGaussianPyramid / buildDoGPyramid (sift.dispatch.cpp:176-310).  7680 ... 120 wide octaves (W % 8 == 0): bit for bit, all levels."""
     from oracle.api import unpack_pyramid
     img = smooth_img(rng, 2160, 3840)

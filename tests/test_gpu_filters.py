@@ -58,14 +58,14 @@ def test_gaussian_u8_rect_kernel_and_batch(cvb, oracle, rng):
 
 
 def test_gaussian_u8_1080p_c3(cvb, ref, rng):
-    """BASELINE config C1: GaussianBlur 5x5 on one 1920x1080 CV_8UC3 frame"""
+    """bench.py workload c1: GaussianBlur 5x5 on one 1920x1080 CV_8UC3 frame"""
     img = rand_u8(rng, 1080, 1920, 3)
     assert_exact(cpu(cvb.GaussianBlur(gpu(img), (5, 5), 0)), ref.GaussianBlur(img, (5, 5), 0), "C1")
 
 
 @pytest.mark.parametrize("k", [3, 5, 7, 9, 11, 13, 15, 21, 31])
 def test_gaussian_u8_4k(cvb, ref, rng, k):
-    """BASELINE config C2 (u8 leg) at full size against the real reference"""
+    """bench.py workload c2 (u8 leg) at full size against the real reference"""
     img = rand_u8(rng, 2160, 3840)
     assert_exact(cpu(cvb.GaussianBlur(gpu(img), (k, k), 0)), ref.GaussianBlur(img, (k, k), 0), "4K u8 k=%d" % k)
 
@@ -237,13 +237,13 @@ def test_filter2d(cvb, oracle, rng, k):
             assert_exact_body(gotf, wantf, 8, atol=5e-4, rtol=1e-5, what="filter2D f32 k=%d b=%d" % (k, b))
             assert_exact(cpu(cvb.filter2D(gpu(img), 5, ker, delta=0.75, borderType=b)), oracle.filter2D(img, 5, ker, delta=0.75, borderType=b), "filter2D u8->f32 k=%d" % k) \
                 if k * k < 50 else None
-        else:               # reference = float DFT, GPU = 3 x BF16 on tcgen05: the reference's own bar for this regime, 1e-4 of the range (test_filter.cpp:420-425)
+        else:               # reference = float DFT, GPU = 3 x BF16 on the tensor cores: the reference's own bar for this regime, 1e-4 of the range (test_filter.cpp:420-425)
             assert_close(gotf, wantf, atol=1e-4 * float(np.abs(wantf).max()), what="filter2D f32 k=%d b=%d" % (k, b))
             assert float(np.abs(gotf - wantf).mean()) <= 2e-5 * float(np.abs(wantf).max()), "filter2D f32 k=%d b=%d: mean error" % (k, b)
 
 
 def test_filter2d_tensor_core(cvb, oracle, rng, monkeypatch):
-    """8-bit filter2D with >= 11x11 taps runs on the tcgen05 correlation engine (three base-256 digit planes of the fixed-point
+    """8-bit filter2D with >= 11x11 taps runs on the tensor-core correlation engine (three base-256 digit planes of the fixed-point
     taps, exact integer MMA).  Checked against the CPU (DFT path) and against our own direct-sum kernel; ragged sizes, several
     M/N tiles and frames, signed taps, off-centre anchor, delta, every destination depth."""
     import os
@@ -268,7 +268,7 @@ def test_filter2d_tensor_core(cvb, oracle, rng, monkeypatch):
 
 
 def test_filter2d_tensor_core_f32(cvb, oracle, rng, monkeypatch):
-    """float filter2D with >= 130 taps runs 3 x BF16 on tcgen05 (FP32 accumulators in TMEM).  Checked against the CPU (its DFT path) at the
+    """float filter2D with >= 130 taps runs 3 x BF16 on the tensor cores (wgmma, FP32 accumulators).  Checked against the CPU (its DFT path) at the
     reference's own bar for that regime (1e-4 of the value range, test_filter.cpp:420-425) and, much tighter on average, against our own
     direct FP32 sum; ragged sizes, several M/N tiles and frames, signed taps, off-centre anchors, delta, non-integer and negative data."""
     img = ((rng.random((3, 301, 263, 1)) - 0.3) * 300).astype(np.float32)
@@ -280,16 +280,16 @@ def test_filter2d_tensor_core_f32(cvb, oracle, rng, monkeypatch):
             monkeypatch.setenv("B200CV_FILTER2D_PATH", "direct")
             direct = cpu(cvb.filter2D(gpu(img), -1, ker, anchor=anchor, delta=delta, borderType=b))
             monkeypatch.delenv("B200CV_FILTER2D_PATH")
-            if kh < 13:         # fewer than 13 kernel rows: the direct FP32 sum is at least as fast and stays (bit-exact path)
+            if kh < 14:         # fewer than 14 kernel rows: the direct FP32 sum is faster and stays (bit-exact path)
                 assert_exact(got, direct, "filter2D f32 %dx%d b=%d stays on the direct sum" % (kh, kw, b))
                 continue
             scale = float(np.abs(direct).max())
-            assert_close(got, direct, atol=1e-4 * scale, what="filter2D f32 tcgen05 vs direct %dx%d b=%d" % (kh, kw, b))
-            assert float(np.abs(got - direct).mean()) <= 1e-5 * scale, "filter2D f32 tcgen05 vs direct %dx%d b=%d: mean error" % (kh, kw, b)
+            assert_close(got, direct, atol=1e-4 * scale, what="filter2D f32 tensor cores vs direct %dx%d b=%d" % (kh, kw, b))
+            assert float(np.abs(got - direct).mean()) <= 1e-5 * scale, "filter2D f32 tensor cores vs direct %dx%d b=%d: mean error" % (kh, kw, b)
             assert (got != direct).mean() > 0.5, "the tensor-core path did not run (results identical to the direct sum)"
             for i in range(img.shape[0]):
                 assert_close(got[i, :, :, 0], oracle.filter2D(img[i, :, :, 0], -1, ker, anchor=anchor, delta=delta, borderType=b), atol=1e-4 * scale,
-                             what="filter2D f32 tcgen05 vs cpu %dx%d b=%d" % (kh, kw, b))
+                             what="filter2D f32 tensor cores vs cpu %dx%d b=%d" % (kh, kw, b))
 
 
 @pytest.mark.parametrize("ksz", [(3, 3), (5, 5), (9, 9), (7, 3), (3, 13), (21, 21)])
@@ -317,8 +317,8 @@ def test_filter2d_tma_path(cvb, oracle, rng, ksz, monkeypatch):
         v1f = cpu(cvb.filter2D(fview, -1, ker, delta=1.25, borderType=b))
         if kw * kh < 130:
             assert_exact(gotf, v1f, "filter2D tma vs v1 f32 %s b=%d" % (ksz, b))
-        else:               # float images with >= 130 taps run 3 x BF16 on tcgen05: against our own direct FP32 sum
-            assert_close(gotf, v1f, atol=1e-4 * float(np.abs(v1f).max()), what="filter2D tcgen05 vs v1 f32 %s b=%d" % (ksz, b))
+        else:               # float images with >= 130 taps run 3 x BF16 on the tensor cores: against our own direct FP32 sum
+            assert_close(gotf, v1f, atol=1e-4 * float(np.abs(v1f).max()), what="filter2D tensor cores vs v1 f32 %s b=%d" % (ksz, b))
         monkeypatch.delenv("B200CV_FILTER2D_PATH")
         for i in range(2):
             want = oracle.filter2D(img[i, :, :, 0], -1, ker, delta=1.25, borderType=b)
@@ -330,7 +330,7 @@ def test_filter2d_tma_path(cvb, oracle, rng, ksz, monkeypatch):
         if kw * kh < 130:
             assert_exact_body(gotf, wantf, 8, atol=5e-4, rtol=1e-5, what="filter2D tma f32 %s b=%d" % (ksz, b))
         else:
-            assert_close(gotf, wantf, atol=1e-4 * float(np.abs(wantf).max()), what="filter2D tcgen05 f32 %s b=%d" % (ksz, b))
+            assert_close(gotf, wantf, atol=1e-4 * float(np.abs(wantf).max()), what="filter2D tensor cores f32 %s b=%d" % (ksz, b))
         if kw * kh < 50:
             assert_exact(got32[0, :, :, 0], oracle.filter2D(img[0, :, :, 0], 5, ker, borderType=b), "filter2D tma u8->f32 %s b=%d" % (ksz, b))
 
@@ -344,8 +344,8 @@ def test_filter2d_generic(cvb, oracle, rng):
 
 @pytest.mark.parametrize("k", [3, 5, 7, 9])
 def test_gaussian_u8_streaming_kernel(cvb, oracle, rng, monkeypatch, k):
-    """the warp-streaming second version of the 8-bit Gaussian (gauss_u8_march.cu; B200CV_GAUSS_U8_PATH=stream -- the tile kernel is the faster
-    one on a B200 and stays the default): bit-exact like the default path, every border, ragged sizes, a batch, and sepFilter2D's 8.8 mode"""
+    """the warp-streaming second version of the 8-bit Gaussian (gauss_u8_march.cu; B200CV_GAUSS_U8_PATH=stream -- the tile kernel
+    stays the default): bit-exact like the default path, every border, ragged sizes, a batch, and sepFilter2D's 8.8 mode"""
     monkeypatch.setenv("B200CV_GAUSS_U8_PATH", "stream")
     for shape in ((3, 211, 333, 1), (1, 64, 224, 1), (2, 37, 1000, 1)):
         img = rng.integers(0, 256, shape, dtype=np.uint8)

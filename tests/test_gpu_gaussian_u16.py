@@ -1,6 +1,6 @@
-"""GPU parity: cv::GaussianBlur on CV_16U images (16.16 fixed point, SURVEY 8(a1)): BIT-EXACT.
+"""GPU parity: cv::GaussianBlur on CV_16U images (16.16 fixed point): BIT-EXACT.
 
-First ran green on a B200 in round 1 (GPUTEST_r01.json); a failure here fails the suite."""
+A failure here fails the suite."""
 import numpy as np
 import pytest
 

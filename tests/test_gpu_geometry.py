@@ -68,7 +68,7 @@ def test_resize_half_area(cvb, oracle, rng, interp):
 @pytest.mark.parametrize("dsize,interp", [((3840, 2160), C.INTER_NEAREST), ((3840, 2160), C.INTER_LINEAR), ((5120, 2880), C.INTER_LINEAR),
                                           ((5120, 2880), C.INTER_CUBIC), ((5120, 2880), C.INTER_NEAREST)])
 def test_resize_8k(cvb, ref, rng, dsize, interp):
-    """BASELINE config C3 (resize leg): 7680x4320 8UC3 source"""
+    """bench.py workload c3 (resize leg): 7680x4320 8UC3 source"""
     img = rand_u8(rng, 4320, 7680, 3)
     assert_exact(cpu(cvb.resize(gpu(img), dsize, interpolation=interp)), ref.resize(img, dsize, interp), "8K -> %s interp %d" % (dsize, interp))
 
@@ -196,7 +196,7 @@ def test_sift_upsample_warp(cvb, oracle, rng):
 
 @pytest.mark.parametrize("interp", [C.INTER_NEAREST, C.INTER_LINEAR, C.INTER_CUBIC])
 def test_warp_8k(cvb, ref, rng, interp):
-    """BASELINE config C3 (warp leg): 7680x4320 8UC3, rotation 7 deg x0.9 about the centre; projective H"""
+    """bench.py workload c3 (warp leg): 7680x4320 8UC3, rotation 7 deg x0.9 about the centre; projective H"""
     img = rand_u8(rng, 4320, 7680, 3)
     M = ref.getRotationMatrix2D((3840, 2160), 7.0, 0.9)
     for border in (C.BORDER_CONSTANT, C.BORDER_REPLICATE):
@@ -251,7 +251,7 @@ def _test_maps(rng, h, w, sw, sh, kind):
 @pytest.mark.parametrize("cn", [1, 3, 4])
 @pytest.mark.parametrize("interp", [C.INTER_NEAREST, C.INTER_LINEAR, C.INTER_CUBIC])
 def test_remap(cvb, oracle, rng, cn, interp):
-    """cv::remap (SURVEY 8f): float x/y planes, packed CV_32FC2 maps and the fixed-point pair of cv::convertMaps; u8 and f32; every border;
+    """cv::remap: float x/y planes, packed CV_32FC2 maps and the fixed-point pair of cv::convertMaps; u8 and f32; every border;
     NaN / out-of-range map values follow x86 cvRound (0x80000000).  Bit-exact."""
     for dt in (np.uint8, np.float32):
         src = (rng.random((97, 131, cn) if cn > 1 else (97, 131)) * 255).astype(dt)
@@ -277,7 +277,7 @@ def test_remap(cvb, oracle, rng, cn, interp):
 
 @pytest.mark.parametrize("shape", [(97, 131), (64, 80), (5, 7), (2, 2), (1, 9), (33, 1), (40, 51, 3), (20, 22, 4), (270, 481, 3)])
 def test_pyramids(cvb, oracle, rng, shape):
-    """cv::pyrDown / cv::pyrUp (SURVEY 8f).  8-bit: bit-exact, every border mode the reference accepts.  Float: bit-exact for pyrUp; for
+    """cv::pyrDown / cv::pyrUp.  8-bit: bit-exact, every border mode the reference accepts.  Float: bit-exact for pyrUp; for
     pyrDown the reference's first / last columns and vector remainders use its scalar operation order (1 ulp): exact inside, 1e-4 there."""
     for dt in (np.uint8, np.float32):
         src = (rng.random(shape) * 255).astype(dt)

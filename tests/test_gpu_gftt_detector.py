@@ -1,7 +1,7 @@
 """GPU: cv::GFTTDetector, the Feature2D wrapper over goodFeaturesToTrack (features2d/src/gftt.cpp:131-148).  It only composes calls that
 tests/test_gpu_features.py verifies (cvtColor + goodFeaturesToTrack).
 
-First ran green on a B200 in round 1 (GPUTEST_r01.json); a failure here fails the suite."""
+A failure here fails the suite."""
 import numpy as np
 import pytest
 

@@ -89,7 +89,7 @@ def test_host_batch_pipeline(cvb, oracle, rng):
 def test_opencv_built_with_b200_hal(cvb, ref, rng):
     """oracle/_ref/libocvref_hal.so is the UNMODIFIED reference compiled with hal/b200cv_hal_replacement.hpp registered as its imgproc
     HAL (what -DOpenCV_HAL_DIR=<repo>/hal does): plain cv::resize / cv::cvtColor / cv::warpAffine / cv::sepFilter2D / cv::GaussianBlur
-    calls on host cv::Mat data now run on the B200 and still return the reference's bytes."""
+    calls on host cv::Mat data now run on the GPU and still return the reference's bytes."""
     from oracle.api import Oracle, available
     if not available("ref_hal"):
         pytest.skip("libocvref_hal.so not built (python oracle/build_ref.py --hal)")
@@ -178,15 +178,15 @@ def test_cpp_host_mirror(cvb):
 
 
 def test_cv_typed_surface_against_real_opencv_headers(cvb):
-    """tests/cpp/test_cv_surface: opencv_b200/host/b200cv_opencv.hpp compiled with -DB200CV_WITH_OPENCV against the reference's own headers and
-    linked with the reference's core + imgproc (built here by tests/cpp/build_cv_surface.py): cv::InputArray kinds MAT / CUDA_GPU_MAT /
+    """oracle/_ref/test_cv_surface: opencv_b200/host/b200cv_opencv.hpp compiled with -DB200CV_WITH_OPENCV against the reference's own headers and
+    linked with the reference's core + imgproc (built by oracle/build_cv_surface.py where the reference's sources are): cv::InputArray kinds MAT / CUDA_GPU_MAT /
     CUDA_HOST_MEM, createGaussianFilter(...)->apply(src, dst, stream) as in gpu-basics-similarity.cpp:392-404, each result checked against
     the cv:: call on the CPU inside the binary"""
     import os
     import subprocess
-    exe = os.path.join(os.path.dirname(__file__), "cpp", "test_cv_surface")
+    exe = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref", "test_cv_surface")
     if not os.path.exists(exe):
-        pytest.skip("tests/cpp/test_cv_surface not built (needs /root/reference at build time)")
+        pytest.skip("oracle/_ref/test_cv_surface not built (needs the reference's sources at build time)")
     r = subprocess.run([exe], capture_output=True, text=True, timeout=300)
     assert r.returncode == 0, r.stdout + r.stderr
     assert "cv surface ok" in r.stdout

@@ -1,6 +1,6 @@
 """GPU parity: cv::integral, 8UC1 -> 32S sum (+ 64F sum of squares): BIT-EXACT (integers; the doubles hold integers below 2^53).
 
-First ran green on a B200 in round 1 (GPUTEST_r01.json); a failure here fails the suite."""
+A failure here fails the suite."""
 import numpy as np
 import pytest
 

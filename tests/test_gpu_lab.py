@@ -1,6 +1,6 @@
 """GPU parity: cv::cvtColor BGR / RGB <-> Lab (sRGB and linear) and <-> CIE XYZ, 8-bit: BIT-EXACT on the whole 2^24 colour cube.
 
-First ran green on a B200 in round 1 (GPUTEST_r01.json); a failure here fails the suite."""
+A failure here fails the suite."""
 import numpy as np
 import pytest
 

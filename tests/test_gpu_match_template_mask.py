@@ -1,7 +1,7 @@
 """GPU: cv::matchTemplate with a mask (all six methods; 8-bit binarised and float weight masks), against the reference at its own bar for
 matchTemplate (1e-3 of the result range; the reference's numerators come from a float DFT, the device sums are direct and in double).
 
-First ran green on a B200 in round 1 (GPUTEST_r01.json); a failure here fails the suite."""
+A failure here fails the suite."""
 import numpy as np
 import pytest
 

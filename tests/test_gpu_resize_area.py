@@ -1,6 +1,6 @@
 """GPU parity: cv::resize INTER_AREA in its true area mode (both factors >= 1), integer and fractional factors, 8-bit and float: BIT-EXACT.
 
-First ran green on a B200 in round 1 (GPUTEST_r01.json); a failure here fails the suite."""
+A failure here fails the suite."""
 import numpy as np
 import pytest
 
@@ -24,7 +24,7 @@ def test_area_resize(cvb, oracle, rng, ssize, dsize, cn):
 
 
 def test_area_resize_8k_batch(cvb, ref, rng):
-    """BASELINE c3 geometry with INTER_AREA: 4 frames 7680x4320 8UC3 -> 5120x2880 (factor 1.5) and -> 2560x1440 (factor 3) in one launch each"""
+    """bench.py workload c3 geometry with INTER_AREA: 4 frames 7680x4320 8UC3 -> 5120x2880 (factor 1.5) and -> 2560x1440 (factor 3) in one launch each"""
     base = rng.integers(0, 256, (4320, 7680, 3), dtype=np.uint8)
     batch = np.stack([np.roll(base, 11 * i, axis=1) for i in range(2)])
     for dsize in ((5120, 2880), (2560, 1440)):

@@ -1,6 +1,6 @@
 """GPU parity: cv::resize INTER_LINEAR_EXACT (8-bit, 8.8 fixed point) and INTER_NEAREST_EXACT (16.16 pixel-centre coordinates): BIT-EXACT.
 
-First ran green on a B200 in round 1 (GPUTEST_r01.json); a failure here fails the suite."""
+A failure here fails the suite."""
 import numpy as np
 import pytest
 
@@ -34,7 +34,7 @@ def test_reference_goldens(cvb):
 
 
 def test_exact_resizers_8k(cvb, ref, rng):
-    """BASELINE c3 geometry: 7680x4320 8UC3 -> 5120x2880 and 3840x2160 (LINEAR_EXACT 2 x 2 = the area fast path)"""
+    """bench.py workload c3 geometry: 7680x4320 8UC3 -> 5120x2880 and 3840x2160 (LINEAR_EXACT 2 x 2 = the area fast path)"""
     img = rng.integers(0, 256, (4320, 7680, 3), dtype=np.uint8)
     for dsize in ((5120, 2880), (3840, 2160)):
         for interp in (C.INTER_LINEAR_EXACT, C.INTER_NEAREST_EXACT):

@@ -1,6 +1,6 @@
 """GPU parity: cv::resize INTER_LANCZOS4, 8-bit and float: BIT-EXACT (weights built on the host with the reference's expressions and libm).
 
-First ran green on a B200 in round 1 (GPUTEST_r01.json); a failure here fails the suite."""
+A failure here fails the suite."""
 import numpy as np
 import pytest
 

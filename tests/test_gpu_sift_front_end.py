@@ -1,4 +1,4 @@
-"""GPU: the SIFT front end after the pyramid -- scale-space extrema, refinement, orientation, descriptors (SURVEY 8(f) rank 1) -- against the
+"""GPU: the SIFT front end after the pyramid -- scale-space extrema, refinement, orientation, descriptors -- against the
 reference's own cv::SIFT::detectAndCompute (enable_precise_upscale = true, the first octave b200cv_sift_pyramid builds).
 
 Parity is by tolerance: the reference's SIFT objects are FMA-contracted AVX2 / AVX-512 builds with OpenCV's approximate exp / atan2, and the small
@@ -7,7 +7,7 @@ reference's keypoints matched to 1e-2 px / 0.1 deg, and for matched keypoints >=
 The port (oracle/port) is pinned to the reference at 99 % / 1e-3 px on the reference's own pyramids (tests/test_oracle.py), and the kernels run on
 the host equal the port exactly (tests/test_kernel_emulation.py).
 
-First ran green on a B200 in round 1 (GPUTEST_r01.json); a failure here fails the suite."""
+A failure here fails the suite."""
 import numpy as np
 import pytest
 
@@ -86,7 +86,7 @@ def test_sift_detect_and_compute(cvb, ref, rng, size):
 
 
 def test_sift_detect_4k(cvb, ref, rng):
-    """BASELINE config C5 frame size: detectAndCompute on one 3840x2160 8UC1 frame against cv::SIFT (sift.dispatch.cpp:176-310, 405-472)"""
+    """bench.py workload c5 frame size: detectAndCompute on one 3840x2160 8UC1 frame against cv::SIFT (sift.dispatch.cpp:176-310, 405-472)"""
     img = structured(rng, 2160, 3840)
     kr, octr, dr = ref.sift_detect_and_compute(img)
     kg, octg, dg = cvb.sift_detectAndCompute(gpu(img))

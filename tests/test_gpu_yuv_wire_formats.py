@@ -2,7 +2,7 @@
 BGR family -> I420 / YV12) through the device C ABI, the host API and the HAL seam.  All integer: BIT-EXACT, checked against the reference's
 own known-answer hashes (modules/imgproc/test/test_color.cpp:2857-2900; inputs = its RNG(0) stream, tests/golden/) and the oracle.
 
-First ran green on a B200 in round 1 (GPUTEST_r01.json); a failure here fails the suite."""
+A failure here fails the suite."""
 import os
 import zlib
 

@@ -343,12 +343,8 @@ def depth_emu():
     return run
 
 
-def test_emulated_depth_cvtcolor_vs_reference(depth_emu, rng):
+def test_emulated_depth_cvtcolor_vs_reference(depth_emu, ref, rng):
     """the kernel source of cvtcolor_depth.cu compiled for the host == the compiled reference, bit for bit (vector bodies and scalar tails)"""
-    from oracle.api import Oracle, available
-    if not available("ref"):
-        pytest.skip("oracle/_ref/libocvref.so not built")
-    ref = Oracle("ref")
     for (h, w) in [(9, 29), (5, 64), (3, 7)]:
         f3 = (rng.random((h, w, 3), dtype=np.float32) * 1.5 - 0.25).astype(np.float32)
         w3 = rng.integers(0, 65536, (h, w, 3), dtype=np.uint16)
@@ -366,11 +362,7 @@ def test_emulated_depth_cvtcolor_vs_reference(depth_emu, rng):
         assert np.array_equal(depth_emu(g, 8, 3), ref.cvtColor(g, 8, 3)) and np.array_equal(depth_emu(g.astype(np.float32), 9, 4), ref.cvtColor(g.astype(np.float32), 9, 4))
 
 
-def test_emulated_bayer_edge_aware_and_16bit_vs_reference(rng):
-    from oracle.api import Oracle, available
-    if not available("ref"):
-        pytest.skip("oracle/_ref/libocvref.so not built")
-    ref = Oracle("ref")
+def test_emulated_bayer_edge_aware_and_16bit_vs_reference(ref, rng):
     lib = build_emulation("demosaic.cu", "int emu_demosaic_any(const b200cvMat* s, const b200cvMat* d, int code)",
                           "    return b200cv::demosaic_bilinear(s, d, code, nullptr);")
     lib.emu_demosaic_any.argtypes = [ctypes.POINTER(Mat), ctypes.POINTER(Mat), ctypes.c_int]

@@ -389,7 +389,7 @@ def test_port_vs_reference_lanczos4_resize(ref, port, rng):
 
 
 def test_reference_sift_front_end_is_reachable(ref, rng):
-    """the oracle for SURVEY 8(f) rank 1: cv::SIFT::detectAndCompute of the unmodified reference (keypoints + 128-float descriptors)"""
+    """the oracle for the SIFT front end: cv::SIFT::detectAndCompute of the unmodified reference (keypoints + 128-float descriptors)"""
     small = rng.random((30, 40)).astype(np.float32)
     img = (np.kron(small, np.ones((8, 8), np.float32)) * 255).astype(np.uint8)
     kp, octv, desc = ref.sift_detect_and_compute(img)
@@ -444,7 +444,7 @@ def test_port_sift_pyramid_default_first_octave(ref, port, rng):
 
 
 def test_port_sift_detector_and_descriptors_vs_reference(ref, port, rng):
-    """SURVEY 8(f) rank 1: scale-space extrema + refinement + orientation + descriptors, restated; fed the reference's own pyramids so that only
+    """The SIFT front end: scale-space extrema + refinement + orientation + descriptors, restated; fed the reference's own pyramids so that only
     this stage is compared.  The reference's SIFT objects are FMA-contracted AVX2 / AVX-512 builds with OpenCV's approximate exp / atan2: the
     agreement is by tolerance.  Measured: >= 99% of the keypoints agree to 1e-3 px / 1e-2 deg (typically all but a handful of borderline
     accept / reject decisions, differences ~3e-5 px); descriptors of identical keypoints differ in < 1e-4 of their entries, by 1."""

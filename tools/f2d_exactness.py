@@ -1,4 +1,4 @@
-"""how many pixels of 8-bit filter2D differ from the reference CPU result: direct FP32 kernel vs tcgen05 fixed-point path"""
+"""how many pixels of 8-bit filter2D differ from the reference CPU result: direct FP32 kernel vs tensor-core fixed-point path"""
 import os
 import sys
 
