@@ -23,10 +23,26 @@
 // Roles (320 threads, one persistent CTA per SM):
 //   warp 8      A producer: per tile the hi and lo strips (K columns x 256 + kh - 1 rows) by TMA in the K-major no-swizzle core-matrix
 //               layout (one 16-byte-wide box column per 8 K elements), ring of 2 stages
-//   warp 9      B producer: one kernel row of Toeplitz operands (8 KB) per cp.async.bulk into a ring of 4, in the order the consumers use them
+//   warp 9      B producer: one kernel row of Toeplitz operands (8 KB) per cp.async.bulk into a ring of FF_NB = 7, in the order the
+//               consumers use them
 //   warps 0-7   two consumer warpgroups of 128 tile rows each: kh x K/16 x 2 slabs x 2 wgmma per tile; a kernel row's A operand is the
-//               same strip with the descriptor start address advanced by one 16-byte row; a B stage is released as soon as the next kernel
-//               row's MMAs are in flight; the epilogue stores from the registers
+//               same strip with the descriptor start address advanced by one 16-byte row; a B stage is released (by both warpgroups) as
+//               soon as the next kernel row's MMAs are in flight
+// Order.  The accumulators live in registers, so a warpgroup's epilogue cannot overlap its own next MMAs; the other warpgroup has to keep
+// the tensor pipe busy meanwhile.  Both warpgroups share each A strip and each streamed B kernel row, so B is read from L2 once per
+// 256-row strip (about 30 B per output pixel at 31 x 31).  Giving each warpgroup its own 128-row tile would double that; starting
+// warpgroup 1 half a tile late would need half a tile of B rows (about 128 KB) resident.  Instead warpgroup 1 starts every tile
+// FF_LAG = 3 kernel rows behind warpgroup 0: warpgroup 0 arrives on lag_bar once it has issued those rows, and warpgroup 1 waits on
+// it before its first MMA.  (An mbarrier rather than a named barrier: the arrive sits between wgmma groups in flight, where only a
+// predicated mbarrier arrive leaves the MMAs unserialised.)  So warpgroup 0 reaches its epilogue 3 kernel rows (about 1.3 k cycles of
+// MMAs at K = 64) before warpgroup 1 does, and warpgroup 1 stores while warpgroup 0 starts the next tile: at most one warpgroup is
+// in its epilogue as long as the epilogue is shorter than that.  The ring holds the lag plus the 4 stages of before.  Measured on an
+// H100 80GB HBM3 at a 400 W power limit (bench.py c2, 8 4K frames): 15 x 15 taps 0.78 ms, 21 x 21 1.13 ms, 31 x 31 1.52 ms, against
+// 0.86 / 1.23 / 1.60 ms with both warpgroups in step and storing from registers.
+// Epilogue.  Per 64-row slab the warpgroup writes its sums into a staging area in shared memory and stores whole 128-byte tile rows
+// with 16-byte stores (element stores only at the right edge or for an unaligned destination).
+// mbarriers: a_full/a_empty[2], b_full/b_empty[7], lag_bar[2] (by tile parity).  Named barriers 1, 2: the staging area of warpgroup
+// 0, 1.
 // The border-extended BF16 planes are written once per call by pad_split_kernel (reads 4 B, writes 4 B per pixel).
 #include <algorithm>
 #include <cmath>
@@ -44,7 +60,11 @@ constexpr int FF_WG = 2;                      // consumer warpgroups, 128 tile r
 constexpr int FF_THREADS = 128 * FF_WG + 64;  // consumer warpgroups, A producer warp, B producer warp
 constexpr int FF_SMEM_MAX = 227 * 1024 - 1024;
 constexpr int FF_NA = 2;                      // A stages
-constexpr int FF_NB = 4;                      // B stages (kernel rows in flight)
+constexpr int FF_LAG = 3;                     // kernel rows warpgroup 1 starts each tile behind warpgroup 0
+constexpr int FF_NB = FF_LAG + 4;             // B stages (kernel rows in flight)
+constexpr int FF_SST = FF_N * 4 + 16;         // epilogue staging row pitch (16 B of padding: fewer bank conflicts)
+constexpr int FF_STAGE = 64 * FF_SST;         // staging bytes per warpgroup (one 64-row slab)
+constexpr int FF_BAR_EPI = 1;                 // named barriers 1, 2: the staging area of warpgroup 0, 1
 
 struct FFTaps { float k[33 * 33]; };
 
@@ -52,6 +72,7 @@ struct FFParams {
     int kh, kch;                              // kernel rows; 16-byte K chunks per plane (K = 8 * kch, even)
     int ra_alloc, box_h, nbox;
     int ow, oh, frames, tiles_x, tiles_y, ntiles;
+    int vec;                                  // destination rows and frames 16-byte aligned: whole-row 16-byte stores
     float delta;
 };
 
@@ -118,12 +139,14 @@ __global__ void __launch_bounds__(FF_THREADS, 1) filter2d_tc_f32_kernel(const __
     const uint32_t abytes = 2 * aplane;                                      // one A stage (hi + lo)
     unsigned char* sB = smem;                                                // FF_NB stages of one kernel row
     unsigned char* sA = smem + (size_t)FF_NB * brow;                         // FF_NA stages
-    __shared__ __align__(8) uint64_t b_full[FF_NB], b_empty[FF_NB], a_full[FF_NA], a_empty[FF_NA];
+    unsigned char* sE = sA + (size_t)FF_NA * abytes;                         // epilogue staging, one slab per warpgroup
+    __shared__ __align__(8) uint64_t b_full[FF_NB], b_empty[FF_NB], a_full[FF_NA], a_empty[FF_NA], lag_bar[2];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < FF_NB; s++) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], 4 * FF_WG); }
         for (int s = 0; s < FF_NA; s++) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 4 * FF_WG); }
+        for (int s = 0; s < 2; s++) mbar_init(&lag_bar[s], 4);
         fence_barrier_init();
     }
     __syncthreads();
@@ -163,7 +186,9 @@ __global__ void __launch_bounds__(FF_THREADS, 1) filter2d_tc_f32_kernel(const __
     }
 
     // ---- consumers: warpgroup wg owns tile rows 128 wg .. 128 wg + 127 as two 64-row slabs ----
-    const int wg = warp >> 2, wl = warp & 3;
+    const int wg = warp >> 2, wl = warp & 3, tid = threadIdx.x & 127;
+    const int lag = min(FF_LAG, p.kh);
+    unsigned char* st = sE + wg * FF_STAGE;
     const uint32_t b_base = smem_u32(sB);
     int i = 0, g = 0;
     for (int t = blockIdx.x; t < p.ntiles; t += gridDim.x, i++) {
@@ -178,6 +203,7 @@ __global__ void __launch_bounds__(FF_THREADS, 1) filter2d_tc_f32_kernel(const __
             for (int r = 0; r < FF_N / 2; r++) alo[m][r] = 0.f;
         }
         mbar_wait(&a_full[buf], (i / FF_NA) & 1);
+        if (wg == 1) mbar_wait(&lag_bar[i & 1], (i >> 1) & 1);     // warpgroup 0 has issued the first `lag` kernel rows of this tile
         wg_fence();
         const uint32_t a0 = smem_u32(sA + (size_t)buf * abytes) + (uint32_t)(wg * 128) * 16u;
         int prev = -1;
@@ -196,6 +222,7 @@ __global__ void __launch_bounds__(FF_THREADS, 1) filter2d_tc_f32_kernel(const __
                 }
             }
             wg_commit();
+            wg_mbar_arrive_if(&lag_bar[i & 1], wg == 0 && lane == 0 && v == lag - 1);
             wg_wait<1>();                            // the previous kernel row's MMAs are done: its B stage may be refilled
             wg_mbar_arrive_if(&b_empty[prev < 0 ? 0 : prev], lane == 0 && prev >= 0);
             prev = s;
@@ -207,22 +234,36 @@ __global__ void __launch_bounds__(FF_THREADS, 1) filter2d_tc_f32_kernel(const __
         wg_fence_operand(alo[1]);
         wg_mbar_arrive_if(&b_empty[prev], lane == 0);
         wg_mbar_arrive_if(&a_empty[buf], lane == 0);
-        // ---- epilogue: hi x hi + lo x hi + hi x lo + delta ----
+        // ---- epilogue: hi x hi + lo x hi + hi x lo + delta, per 64-row slab through the staging area, whole 128-byte rows out ----
 #pragma unroll
-        for (int m = 0; m < 2; m++)
+        for (int m = 0; m < 2; m++) {
+            wg_bar_sync(FF_BAR_EPI + wg, 128);                 // the staging area's previous contents are stored
 #pragma unroll
             for (int ii = 0; ii < 2; ii++) {
-                const int gy = ty * (128 * FF_WG) + wg * 128 + m * 64 + wl * 16 + (lane >> 2) + 8 * ii;
-                if (gy >= p.oh) continue;
-                float* dp = dst.row<float>(f, gy);
+                const int row = wl * 16 + (lane >> 2) + 8 * ii;
 #pragma unroll
-                for (int j = 0; j < FF_N / 8; j++)
+                for (int j = 0; j < FF_N / 8; j++) {
+                    float o[2];
 #pragma unroll
                     for (int c = 0; c < 2; c++) {
-                        const int gx = tx * FF_N + 8 * j + 2 * (lane & 3) + c, r = 4 * j + 2 * ii + c;
-                        if (gx < p.ow) dp[gx] = __fadd_rn(__fadd_rn(__fadd_rn(acc[m][r], alo[m][r]), acc[m][r + FF_N / 2]), p.delta);
+                        const int r = 4 * j + 2 * ii + c;
+                        o[c] = __fadd_rn(__fadd_rn(__fadd_rn(acc[m][r], alo[m][r]), acc[m][r + FF_N / 2]), p.delta);
                     }
+                    *(float2*)(st + row * FF_SST + (8 * j + 2 * (lane & 3)) * 4) = make_float2(o[0], o[1]);
+                }
             }
+            wg_bar_sync(FF_BAR_EPI + wg, 128);
+            for (int idx = tid; idx < 64 * (FF_N / 4); idx += 128) {
+                const int row = idx / (FF_N / 4), c = idx % (FF_N / 4);
+                const int gy = ty * (128 * FF_WG) + wg * 128 + m * 64 + row, gx = tx * FF_N + 4 * c;
+                if (gy >= p.oh) continue;
+                float* gp = dst.row<float>(f, gy) + gx;
+                const float* sp = (const float*)(st + row * FF_SST) + 4 * c;
+                if (p.vec && gx + 4 <= p.ow) *(float4*)gp = *(const float4*)sp;
+                else
+                    for (int e = 0; e < 4 && gx + e < p.ow; e++) gp[e] = sp[e];
+            }
+        }
     }
 }
 
@@ -252,8 +293,9 @@ int filter2d_f32_tensor(const Img& s, const Img& d, const float* k, int kw, int 
     p.box_h = (((ra + p.nbox - 1) / p.nbox) + 7) & ~7;
     p.ra_alloc = p.nbox * p.box_h;
     const size_t brow = (size_t)p.kch * 2 * FF_N * 16, abytes = (size_t)2 * p.kch * p.ra_alloc * 16;
-    const size_t smem = (size_t)FF_NB * brow + FF_NA * abytes;
+    const size_t smem = (size_t)FF_NB * brow + FF_NA * abytes + FF_WG * FF_STAGE;
     if (smem > (size_t)FF_SMEM_MAX) return B200CV_NOT_IMPLEMENTED;
+    p.vec = (((uintptr_t)d.data | d.step | d.fstep) & 15) == 0;
     const int grid = (int)std::min<long long>(nt, num_sms());
 
     // border-extended source as BF16 hi / lo planes, rows padded to a multiple of 8 elements (16 bytes: TMA)

@@ -43,6 +43,15 @@ __device__ __forceinline__ void wg_mbar_arrive_if(uint64_t* bar, bool pred)
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %1, 0;\n\t@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}"
                  ::"r"((uint32_t)__cvta_generic_to_shared(bar)), "r"((uint32_t)pred) : "memory");
 }
+// named barriers (ids 1..15; 0 is __syncthreads) between warpgroups.  `n` counts every thread taking part, arriving and waiting.
+// wg_bar_arrive does not wait.  Between wgmma groups in flight use it unconditionally: even a predicated bar.arrive there makes ptxas
+// serialise the MMAs (C7520).  wg_bar_sync_if takes a `pred` uniform over each warp.
+__device__ __forceinline__ void wg_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void wg_bar_sync_if(int id, int n, bool pred)
+{
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t@p bar.sync %0, %1;\n\t}" ::"r"(id), "r"(n), "r"((uint32_t)pred) : "memory");
+}
+__device__ __forceinline__ void wg_bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 // one bulk copy global -> shared, completion signalled on `bar` with the byte count
 __device__ __forceinline__ void wg_bulk_load(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar)
 {
@@ -58,6 +67,16 @@ __device__ __forceinline__ void wgmma_u8u8_n64(uint32_t (&d)[32], uint64_t adesc
                  : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]),
                    "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
                    "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+                 : "l"(adesc), "l"(bdesc) : "memory");
+}
+
+// D[64 x 48] += A[64 x 32] * B[32 x 48], u8 x s8 -> s32, both operands K-major in shared memory
+__device__ __forceinline__ void wgmma_u8s8_n48(uint32_t (&d)[24], uint64_t adesc, uint64_t bdesc)
+{
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n48k32.s32.u8.s8 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p;\n\t}"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]),
+                   "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23])
                  : "l"(adesc), "l"(bdesc) : "memory");
 }
 
