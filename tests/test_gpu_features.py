@@ -1,8 +1,10 @@
 """GPU parity: matchTemplate, cornerHarris / cornerMinEigenVal, goodFeaturesToTrack, SIFT pyramid vs the CPU oracle.
 
 Bars
-  matchTemplate ......... relative 1e-3 of the result range (the reference's own bar, test_templmatch.cpp:333; its numerator is a
-                          float DFT, ours is the exact integer sum for 8-bit images)
+  matchTemplate ......... relative 1e-3 of the result range against the reference: the reference's own bar (test_templmatch.cpp:333),
+                          set by the round-off of its float DFT numerator.  The exact bars (bit equality for 8-bit TM_CCORR, one
+                          float32 ulp for the other methods, a per-element rounding bound for float images) and the shapes that reach
+                          each numerator kernel live in test_gpu_match_template_exact.py
   cornerHarris/MinEig ... |d| <= 2e-6 * max|ref| + tiny  (reference test: relative 2e-6, test_goodfeaturetotrack.cpp:439-513;
                           operations are the same fp32 ones, only FMA chaining inside the 3-tap Sobel rows differs)
   goodFeaturesToTrack ... identical corner list (order included) whenever the response maps agree on the ranking; compared as
