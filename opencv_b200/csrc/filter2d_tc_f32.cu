@@ -3,11 +3,14 @@
 // (dft_filter_size, filter.dispatch.cpp:1288-1290; its own tolerance there is 1e-4 of the value range, test_filter.cpp:420-425).
 // Smaller kernels stay on the FP32 kernel of filter2d_tma.cu, which reproduces the reference's direct sum bit for bit.
 //
-// Arithmetic: 3 x BF16.  Every float is split into hi = bf16(a) and lo = bf16(a - hi) (|a - hi - lo| <= 2^-16 |a|); the product sum is
+// Arithmetic: 3 x BF16.  Every float is split into hi = bf16(a) and lo = bf16(a - hi) (|a - hi - lo| <= 2^-16 |a|; hi saturates to the
+// largest finite BF16 instead of overflowing, see ff_split); the product sum is
 //   sum a k  ~=  sum a_hi k_hi + sum a_hi k_lo + sum a_lo k_hi        (the dropped a_lo k_lo term is another 2^-16)
 // in FP32 accumulators.  Relative to sum |a| |k| the error is <= ~4e-5 worst case (all signs aligned), ~1e-6 typical -- inside the
 // reference's bar for this regime and below what its float DFT itself loses on 31 x 31 kernels.  BF16 keeps float's exponent range, so
-// no data-dependent scaling (and no reduction pass over the image) is needed.
+// no data-dependent scaling (and no reduction pass over the image) is needed.  A NaN or inf PIXEL is not contained: every padded pixel of
+// a tile's strip meets the Toeplitz zero taps too (inf x 0 = NaN), so it spreads to up to 32 + kw - 1 columns of its output rows (the
+// reference's DFT spreads it over more).
 //
 // Contraction = the Toeplitz form of filter2d_tc.cu / matchtemplate_tc.cu:
 //   D[m][j] = sum_v sum_k A_v[m][k] * B_v[k][j],   A_v[m][k] = P(y0 + m + v, x0 + k),   B_v[k][j] = K(v, k - j)   (0 outside 0 <= k-j < kw)
@@ -76,6 +79,15 @@ struct FFParams {
     float delta;
 };
 
+// hi = bf16(a), lo = bf16(a - hi).  A finite |a| >= 3.3962e38 rounds to a BF16 infinity, which would make lo the opposite infinity and
+// the sums NaN: hi then takes the largest finite BF16 of a's sign, so lo stays finite and |a - hi - lo| <= 2^-16 |a| still holds.
+__device__ __forceinline__ void ff_split(float a, __nv_bfloat16& hi, __nv_bfloat16& lo)
+{
+    hi = __float2bfloat16_rn(a);
+    if (isinf(__bfloat162float(hi)) && !isinf(a)) hi = __ushort_as_bfloat16(a < 0.f ? 0xFF7Fu : 0x7F7Fu);
+    lo = __float2bfloat16_rn(a - __bfloat162float(hi));
+}
+
 // B in global/shared memory: [kernel row v][chunk c][column n (64: 0..31 hi plane, 32..63 lo plane)][8 bf16]: element e of column j = n & 31
 // = plane(K(v, 8c + e - j)): K-major core matrices of 8 columns x 16 bytes, 128 bytes apart in N, 1024 bytes apart in K
 __global__ void ff_toeplitz_kernel(const __grid_constant__ FFTaps kp, int kw, int kch, __nv_bfloat16* out)
@@ -87,8 +99,8 @@ __global__ void ff_toeplitz_kernel(const __grid_constant__ FFTaps kp, int kw, in
         const int pl = n / FF_N, j = n % FF_N;
         const int u = 8 * c + e - j;
         const float t = (u >= 0 && u < kw) ? kp.k[v * kw + u] : 0.f;
-        const __nv_bfloat16 hi = __float2bfloat16_rn(t);
-        const __nv_bfloat16 lo = __float2bfloat16_rn(t - __bfloat162float(hi));
+        __nv_bfloat16 hi, lo;
+        ff_split(t, hi, lo);
         out[(size_t)v * per_row + idx] = pl ? lo : hi;
     }
 }
@@ -117,8 +129,9 @@ __global__ void __launch_bounds__(128) ff_pad_split_kernel(Img src, __nv_bfloat1
     uint32_t hi[4], lo[4];
 #pragma unroll
     for (int i = 0; i < 4; i++) {
-        const __nv_bfloat16 h0 = __float2bfloat16_rn(a[2 * i]), h1 = __float2bfloat16_rn(a[2 * i + 1]);
-        const __nv_bfloat16 l0 = __float2bfloat16_rn(a[2 * i] - __bfloat162float(h0)), l1 = __float2bfloat16_rn(a[2 * i + 1] - __bfloat162float(h1));
+        __nv_bfloat16 h0, h1, l0, l1;
+        ff_split(a[2 * i], h0, l0);
+        ff_split(a[2 * i + 1], h1, l1);
         hi[i] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
         lo[i] = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
     }

@@ -6,6 +6,8 @@ strips shared by both warpgroups, the second one a few kernel rows behind.  The 
 above the SM count (so CTAs have one, two or several tiles, and some warpgroups none), heights that are not multiples of the tile
 height, widths that are not multiples of the tile width, one frame and several, and destinations whose rows are not 16-byte aligned.
 Bars: 1 LSB for 8-bit destinations (exact integer sums; only .5 ties may round differently), the direct sum's own accuracy elsewhere.
+These compare two device paths; tests/test_gpu_filter2d_tc_exact.py holds the tensor-core kernels to an exact restatement of their
+arithmetic (tests/f2d_reference.py), bit for bit for 8-bit sources.
 """
 import numpy as np
 import pytest

@@ -7,7 +7,10 @@ Tolerances
     source) elements of each row are the reference's scalar remainder loops: |d| <= 1e-4 + 1e-5 |ref| there (the reference's own
     bar for the whole image: test_filter.cpp:826-830 uses 1e-5 relative)
   filter2D u8: BIT-EXACT below 130 taps (the CPU's direct float sum, reproduced in operation order); <= 1 LSB from 130 taps on, where
-    the CPU uses a DFT (its own test allows 2, test_filter.cpp:420-425) and the GPU an exact fixed-point tensor-core correlation
+    the CPU uses a DFT (its own test allows 2, test_filter.cpp:420-425) and the GPU an exact fixed-point tensor-core correlation.
+    Against the reference these bars stay; tests/test_gpu_filter2d_tc_exact.py holds both tensor-core kernels (8-bit: bit for bit;
+    float: bit for bit on exactly representable data, a derived per-element bar otherwise) to their own arithmetic, restated in
+    tests/f2d_reference.py
 """
 import numpy as np
 import pytest
