@@ -11,7 +11,9 @@
 // goodFeaturesToTrack (modules/imgproc/src/featureselect.cpp:382-548): response map -> per-frame max (warp-shuffle +
 // atomic reduction) -> threshold at max*quality (TOZERO) -> 3x3 non-maximum test (== dilate + compare) -> compaction of
 // (value, position) candidates on the device; the ordered part (sort by value then address, greedy min-distance
-// acceptance on a cell grid) runs on the host over the compacted list, as it is inherently sequential.
+// acceptance on a cell grid) runs on the host over the compacted list, as it is inherently sequential.  The list holds 2^20 candidates
+// per frame; a frame with more (a noise frame at 8K has ~2 10^6, a plateau frame up to (W - 2)(H - 2)) makes the list grow to the
+// largest count and the candidates be found a second time, so no candidate is ever dropped.
 #include <algorithm>
 #include <chrono>
 #include <cstdio>
@@ -649,7 +651,6 @@ extern "C" int b200cv_good_features_to_track(const b200cvMat* src, float* corner
     TRY(cudaMallocAsync(&d_cnt, sizeof(int) * frames, st));
     TRY(cudaMallocAsync(&d_cand, sizeof(CandKey) * (size_t)cap * frames, st));
     TRY(cudaMemsetAsync(d_max, 0, sizeof(unsigned) * frames, st));
-    TRY(cudaMemsetAsync(d_cnt, 0, sizeof(int) * frames, st));
     b200cvMat eig = {d_eig, pitch, W, H, B200CV_MAKETYPE(B200CV_32F, 1), frames, pitch * H};
     rc = corner_response(src, &eig, block_size, gradient_size, k, B200CV_BORDER_REFLECT_101, use_harris ? 0 : 1, stream);
     if (rc) { cleanup(); return rc; }
@@ -668,27 +669,43 @@ extern "C" int b200cv_good_features_to_track(const b200cvMat* src, float* corner
         TRY(cudaMallocAsync(&d_thr, sizeof(int) * frames, st));
         TRY(cudaMallocAsync(&d_topcnt, sizeof(int) * frames, st));
         TRY(cudaMallocAsync(&d_top, sizeof(CandKey) * (size_t)GF_TOP_CAP * frames, st));
-        TRY(cudaMemsetAsync(d_hist, 0, sizeof(unsigned) * GF_BINS * frames, st));
-        TRY(cudaMemsetAsync(d_topcnt, 0, sizeof(int) * frames, st));
     }
-    {
+    std::vector<int> hcnt(frames), hsel(frames, 0);
+    // candidates (and the preselection) of every frame, then one synchronisation that brings the counts back.  The kernel counts every
+    // candidate but stores only the first `cap` of a frame
+    auto find_candidates = [&]() -> cudaError_t {
+        cudaError_t ce = cudaMemsetAsync(d_cnt, 0, sizeof(int) * frames, st);
+        if (ce == cudaSuccess && preselect) ce = cudaMemsetAsync(d_hist, 0, sizeof(unsigned) * GF_BINS * frames, st);
+        if (ce == cudaSuccess && preselect) ce = cudaMemsetAsync(d_topcnt, 0, sizeof(int) * frames, st);
+        if (ce != cudaSuccess) return ce;
         const unsigned tiles = div_up(W, 1024) * div_up(H, GC_R);
         gftt_candidates_kernel<<<dim3(std::min(tiles, (unsigned)num_sms() * 8u), frames), 256, 0, st>>>(e, d_max, quality_level, d_cand, cap, d_cnt, d_hist);
         count_launch();
-        TRY(cudaGetLastError());
+        if ((ce = cudaGetLastError()) != cudaSuccess) return ce;
+        if (preselect) {
+            gftt_select_kernel<<<frames, 128, 0, st>>>(d_hist, d_thr);
+            gftt_filter_kernel<<<dim3(128, frames), 256, 0, st>>>(d_cand, d_cnt, cap, d_thr, d_top, d_topcnt);
+            count_launch(2);
+            if ((ce = cudaGetLastError()) != cudaSuccess) return ce;
+        }
+        if ((ce = cudaMemcpyAsync(hcnt.data(), d_cnt, sizeof(int) * frames, cudaMemcpyDeviceToHost, st)) != cudaSuccess) return ce;
+        if (preselect && (ce = cudaMemcpyAsync(hsel.data(), d_topcnt, sizeof(int) * frames, cudaMemcpyDeviceToHost, st)) != cudaSuccess) return ce;
+        lap("enqueue 1");
+        ce = cudaStreamSynchronize(st);
+        lap("sync 1");
+        return ce;
+    };
+    TRY(find_candidates());
+    // a frame with more candidates than the list holds (noise or plateaus at 8K: up to (W - 2)(H - 2)): every candidate is kept -- the
+    // list grows to the largest count and the candidates are found again (the common case keeps one pass and the 2^20-entry list)
+    const int most = *std::max_element(hcnt.begin(), hcnt.end());
+    if (most > cap) {
+        TRY(cudaFreeAsync(d_cand, st));
+        d_cand = nullptr;
+        cap = most;
+        TRY(cudaMallocAsync(&d_cand, sizeof(CandKey) * (size_t)cap * frames, st));
+        TRY(find_candidates());
     }
-    if (preselect) {
-        gftt_select_kernel<<<frames, 128, 0, st>>>(d_hist, d_thr);
-        gftt_filter_kernel<<<dim3(128, frames), 256, 0, st>>>(d_cand, d_cnt, cap, d_thr, d_top, d_topcnt);
-        count_launch(2);
-        TRY(cudaGetLastError());
-    }
-    std::vector<int> hcnt(frames), hsel(frames, 0);
-    TRY(cudaMemcpyAsync(hcnt.data(), d_cnt, sizeof(int) * frames, cudaMemcpyDeviceToHost, st));
-    if (preselect) TRY(cudaMemcpyAsync(hsel.data(), d_topcnt, sizeof(int) * frames, cudaMemcpyDeviceToHost, st));
-    lap("enqueue 1");
-    TRY(cudaStreamSynchronize(st));
-    lap("sync 1");
     // order the candidates on the device (library radix sort: not per-pixel work), then walk them on the host in chunks --
     // the greedy minimum-distance selection is sequential and normally stops after a short prefix
     int nmax = 0;

@@ -6,9 +6,13 @@ Bars
                           float32 ulp for the other methods, a per-element rounding bound for float images) and the shapes that reach
                           each numerator kernel live in test_gpu_match_template_exact.py
   cornerHarris/MinEig ... |d| <= 2e-6 * max|ref| + tiny  (reference test: relative 2e-6, test_goodfeaturetotrack.cpp:439-513;
-                          operations are the same fp32 ones, only FMA chaining inside the 3-tap Sobel rows differs)
+                          operations are the same fp32 ones, only FMA chaining inside the 3-tap Sobel rows differs).  The
+                          reference's own box filter uses running sums, so this bar stays; the device's arithmetic is held bit
+                          for bit to a numpy restatement of harris.cu in test_gpu_corner_exact.py (every path, size edge and border)
   goodFeaturesToTrack ... identical corner list (order included) whenever the response maps agree on the ranking; compared as
-                          exact coordinates on inputs with well separated responses
+                          exact coordinates on inputs with well separated responses.  The selection on the device's own map
+                          (positions, order and qualities, ties, the threshold, 8K frames past the first candidate list) is held
+                          exact in test_gpu_corner_exact.py
   SIFT pyramid .......... per level |d| <= 1e-3 absolute on a 0..255 scale (a chain of up to 5 f32 blurs per octave and 10 octaves;
                           NOTE the reference has no test that pins these pyramids -- the oracle is the reference's own code
                           (oracle/_ref) or the same composition of public calls in the port)
