@@ -75,4 +75,6 @@
 #define cv_hal_cvtBGRtoHSV b200cv_hal_cvtBGRtoHSV
 #undef cv_hal_cvtHSVtoBGR
 #define cv_hal_cvtHSVtoBGR b200cv_hal_cvtHSVtoBGR
+#undef cv_hal_canny
+#define cv_hal_canny b200cv_hal_canny
 #endif

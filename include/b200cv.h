@@ -216,6 +216,21 @@ B200CV_API int b200cv_corner_min_eigen_val(const b200cvMat* src, const b200cvMat
 B200CV_API int b200cv_good_features_to_track(const b200cvMat* src, float* corners, float* quality, int max_out,
                                              int* counts, int max_corners, double quality_level, double min_distance,
                                              int block_size, int gradient_size, int use_harris, double k, void* stream);
+/* replaces cv::Canny (imgproc.hpp:1889, :1907; canny.cpp:823-931 and :933-1003), bit-exact.  src: 8-bit, 1-4 channels; dst: 8UC1 of the
+ * source size (src == dst allowed for 8UC1).  aperture_size 3 / 5 / 7, or -1 for Scharr; the legacy CV_CANNY_L2_GRADIENT bit (1 << 31) in
+ * aperture_size turns on L2.  Thresholds are the user's: /16 for aperture 7 and the low/high swap happen here, as in canny.cpp:838-856.
+ * Integer thresholds follow the reference's x86-64 cvFloor ((int)floor(v) by cvttsd2si): a NaN or a value outside the int range, of
+ * either sign, becomes INT_MIN (so an L1 threshold of 1e10 keeps every non-maximum-suppressed maximum).
+ * b200cv_canny_derivs is cv::Canny(dx, dy, ...): dx, dy 16SC1 or 16SC3 of the same type and size (no /16 step).
+ * Scratch: int32 labels from the stream-ordered pool, 4 B per pixel per frame (531 MB for 16 4K frames); W * H must be below 2^31.
+ * Four launches per call, whatever the image holds; nothing synchronises the host.  L1 takes |-32768| as 32768 (the reference's scalar
+ * loop; its SIMD loop differs there, which only Canny(dx, dy) can reach).
+ * Other depths, or derivatives with another channel count: B200CV_NOT_IMPLEMENTED.  A bad aperture, dx / dy that differ, or a dst that is
+ * not 8UC1 of the source size: B200CV_ERR_BAD_ARG, dst untouched. */
+B200CV_API int b200cv_canny(const b200cvMat* src, const b200cvMat* dst, double threshold1, double threshold2, int aperture_size,
+                            int l2gradient, void* stream);
+B200CV_API int b200cv_canny_derivs(const b200cvMat* dx, const b200cvMat* dy, const b200cvMat* dst, double threshold1, double threshold2,
+                                   int l2gradient, void* stream);
 /* SIFT Gaussian pyramid + DoG (features2d/src/sift.dispatch.cpp:176-310).
  * src: 8UC1 batch.  gauss / dog: device float buffers, per frame packed image after image, octave-major
  * (n_octaves*(n_layers+3) Gaussian images, n_octaves*(n_layers+2) DoG images); per-frame strides in floats.

@@ -120,6 +120,11 @@ B200CV_API int b200cv_hal_cvtOnePlaneBGRtoYUV(const b200cv_uchar* src_data, size
 B200CV_API int b200cv_hal_cvtOnePlaneYUVtoBGR(const b200cv_uchar* src_data, size_t src_step, b200cv_uchar* dst_data, size_t dst_step, int width, int height,
                                               int dcn, bool swapBlue, int uIdx, int ycn);
 
+/* hal_ni_canny, hal_replacement.hpp:1291 (cv::Canny, canny.cpp:864): 8-bit, 1-4 channels.  The thresholds arrive already divided by 16
+ * for aperture 7 and swapped (canny.cpp:848-856 runs before the call) and are used as given; ksize 3 / 5 / 7 or -1 (Scharr) */
+B200CV_API int b200cv_hal_canny(const b200cv_uchar* src_data, size_t src_step, b200cv_uchar* dst_data, size_t dst_step, int width, int height,
+                                int cn, double lowThreshold, double highThreshold, int ksize, bool L2gradient);
+
 /* ---- batched host API (what cv::-signature wrappers over cv::Mat call; pipelined over 3 streams) ----------------------- */
 B200CV_API int b200cv_host_gaussian_blur(const b200cvMat* src, const b200cvMat* dst, int ksize_w, int ksize_h, double sigma_x, double sigma_y, int border);
 B200CV_API int b200cv_host_sep_filter2d(const b200cvMat* src, const b200cvMat* dst, const float* kx, int kx_len, const float* ky, int ky_len,
@@ -142,6 +147,8 @@ B200CV_API int b200cv_host_cvt_color(const b200cvMat* src, const b200cvMat* dst,
 B200CV_API int b200cv_host_match_template(const b200cvMat* image, const b200cvMat* templ, const b200cvMat* result, int method);
 B200CV_API int b200cv_host_corner_harris(const b200cvMat* src, const b200cvMat* dst, int block_size, int ksize, double k, int border);
 B200CV_API int b200cv_host_corner_min_eigen_val(const b200cvMat* src, const b200cvMat* dst, int block_size, int ksize, int border);
+/* cv::Canny over host frames; thresholds and aperture as b200cv_canny takes them */
+B200CV_API int b200cv_host_canny(const b200cvMat* src, const b200cvMat* dst, double threshold1, double threshold2, int aperture_size, int l2gradient);
 
 #ifdef __cplusplus
 }

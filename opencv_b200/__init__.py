@@ -4,7 +4,7 @@ The functions mirror the cv2 / cv:: names and argument meaning of the reference
 (modules/imgproc/include/opencv2/imgproc.hpp) for the calls on the hot path:
 
     GaussianBlur, sepFilter2D, filter2D, Sobel, resize, warpAffine, warpPerspective, cvtColor,
-    matchTemplate, cornerHarris, cornerMinEigenVal, goodFeaturesToTrack, sift_pyramid
+    matchTemplate, cornerHarris, cornerMinEigenVal, goodFeaturesToTrack, Canny, sift_pyramid
 
 Inputs are torch CUDA tensors laid out like a cv::Mat -- (H, W) or (H, W, C), or a batch
 (N, H, W[, C]) of independent frames -- and go to the device C ABI (include/b200cv.h) without a
@@ -472,6 +472,49 @@ def cornerMinEigenVal(src, blockSize, ksize=3, borderType=BORDER_DEFAULT, dst=No
     _check(lib().b200cv_corner_min_eigen_val(ctypes.byref(ms), ctypes.byref(md), int(blockSize), int(ksize), int(borderType),
                                              _stream_ptr(stream)), "cornerMinEigenVal")
     return dst
+
+
+def _int32(v):
+    """a Python int as the C int of the same bits (cv2 passes CV_CANNY_L2_GRADIENT = 1 << 31 inside apertureSize)"""
+    return ((int(v) + (1 << 31)) % (1 << 32)) - (1 << 31)
+
+
+def _is_array(x):
+    return _is_torch(x) or isinstance(x, np.ndarray)
+
+
+def Canny(*args, **kwargs):
+    """cv::Canny (imgproc.hpp:1889, :1907), both of cv2's overloads:
+        Canny(image, threshold1, threshold2, edges=None, apertureSize=3, L2gradient=False, stream=None)
+        Canny(dx, dy, threshold1, threshold2, edges=None, L2gradient=False, stream=None)
+    chosen by whether the second argument is an array.  Returns 8-bit edges (0 / 255), one channel, of the input's size."""
+    if (len(args) > 1 and _is_array(args[1])) or "dy" in kwargs:
+        return _canny_derivs(*args, **kwargs)
+    return _canny_image(*args, **kwargs)
+
+
+def _canny_image(image, threshold1, threshold2, edges=None, apertureSize=3, L2gradient=False, stream=None):
+    if not _is_torch(image):
+        from . import hal
+        return hal.Canny(image, threshold1, threshold2, edges, apertureSize, L2gradient)
+    import torch
+    edges = edges if edges is not None else _new(image, dtype=torch.uint8, channels=1)
+    ms, md = _pair(image, edges)
+    _check(lib().b200cv_canny(ctypes.byref(ms), ctypes.byref(md), ctypes.c_double(threshold1), ctypes.c_double(threshold2), _int32(apertureSize),
+                              int(bool(L2gradient)), _stream_ptr(stream)), "Canny")
+    return edges
+
+
+def _canny_derivs(dx, dy, threshold1, threshold2, edges=None, L2gradient=False, stream=None):
+    if not _is_torch(dx):
+        from . import hal
+        return hal.Canny(dx, dy, threshold1, threshold2, edges, L2gradient)
+    import torch
+    edges = edges if edges is not None else _new(dx, dtype=torch.uint8, channels=1)
+    mx, my, md = describe(dx), describe(dy), describe(edges)
+    _check(lib().b200cv_canny_derivs(ctypes.byref(mx), ctypes.byref(my), ctypes.byref(md), ctypes.c_double(threshold1), ctypes.c_double(threshold2),
+                                     int(bool(L2gradient)), _stream_ptr(stream)), "Canny")
+    return edges
 
 
 def goodFeaturesToTrack(image, maxCorners, qualityLevel, minDistance, blockSize=3, gradientSize=3, useHarrisDetector=False, k=0.04,

@@ -157,4 +157,9 @@ int gauss_u8_march(const Img& s, const Img& d, int KB, const unsigned char* tx, 
 int gauss_u8_fast(const Img& s, const Img& d, int cn, const int64_t* fx, int kw, const int64_t* fy, int kh, int border, cudaStream_t st, int sep_mode = 0, int even_limit = 0,
                   const GU8Box* box = nullptr);
 
+// canny.cu: cv::Canny's argument step before its HAL call (L2 bit, aperture check, /16 for aperture 7, swap), and the computation from
+// thresholds that have been through it (dy != NULL: src is dx and the 16S derivatives are given)
+int canny_user_args(double* low, double* high, int* aperture, int* l2);
+int canny_prepared(const b200cvMat* src, const b200cvMat* dy, const b200cvMat* dst, double low, double high, int aperture, int l2, void* stream);
+
 }  // namespace b200cv

@@ -198,6 +198,8 @@ extern "C" int b200cv_host_corner_harris(const b200cvMat* s, const b200cvMat* d,
 { return host_pipeline(s, d, [=](const b200cvMat* a, const b200cvMat* b, void* st) { return b200cv_corner_harris(a, b, bs, ks, k, border, st); }); }
 extern "C" int b200cv_host_corner_min_eigen_val(const b200cvMat* s, const b200cvMat* d, int bs, int ks, int border)
 { return host_pipeline(s, d, [=](const b200cvMat* a, const b200cvMat* b, void* st) { return b200cv_corner_min_eigen_val(a, b, bs, ks, border, st); }); }
+extern "C" int b200cv_host_canny(const b200cvMat* s, const b200cvMat* d, double t1, double t2, int aperture, int l2)
+{ return host_pipeline(s, d, [=](const b200cvMat* a, const b200cvMat* b, void* st) { return b200cv_canny(a, b, t1, t2, aperture, l2, st); }); }
 
 extern "C" int b200cv_host_match_template(const b200cvMat* image, const b200cvMat* templ, const b200cvMat* result, int method)
 {
@@ -505,4 +507,14 @@ extern "C" int b200cv_hal_cvtHSVtoBGR(const uchar* src, size_t sstep, uchar* dst
 {
     if (!isHSV) return B200CV_NOT_IMPLEMENTED;
     return cvt(src, sstep, dst, dstep, w, h, depth, 3, dcn, full ? (swapBlue ? 71 : 70) : (swapBlue ? 55 : 54));
+}
+
+// cv::Canny has already turned the user's arguments into these (canny.cpp:838-856) and dropped the ROI context (:861-862): the thresholds
+// go to the computation as they are
+extern "C" int b200cv_hal_canny(const uchar* src, size_t sstep, uchar* dst, size_t dstep, int w, int h, int cn, double low, double high, int ksize,
+                                bool L2gradient)
+{
+    b200cvMat s = hmat(src, sstep, w, h, B200CV_MAKETYPE(B200CV_8U, cn)), d = hmat(dst, dstep, w, h, B200CV_MAKETYPE(B200CV_8U, 1));
+    const int l2 = L2gradient ? 1 : 0;
+    return host_pipeline(&s, &d, [=](const b200cvMat* a, const b200cvMat* b, void* st) { return canny_prepared(a, nullptr, b, low, high, ksize, l2, st); });
 }

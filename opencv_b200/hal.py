@@ -104,6 +104,37 @@ def Sobel(src, ddepth, dx, dy, ksize=3, scale=1.0, delta=0.0, borderType=BORDER_
     return dst
 
 
+def Canny(*args, **kwargs):
+    """cv::Canny over host arrays, both overloads: Canny(image, threshold1, threshold2, edges=None, apertureSize=3, L2gradient=False) and
+    Canny(dx, dy, threshold1, threshold2, edges=None, L2gradient=False).  The image overload runs b200cv_host_canny; the derivative
+    overload uploads dx and dy and runs b200cv_canny_derivs."""
+    if (len(args) > 1 and isinstance(args[1], np.ndarray)) or "dy" in kwargs:
+        return _canny_derivs(*args, **kwargs)
+    return _canny_image(*args, **kwargs)
+
+
+def _canny_image(image, threshold1, threshold2, edges=None, apertureSize=3, L2gradient=False):
+    from . import _int32
+    edges = edges if edges is not None else _new(image, dtype=np.uint8, channels=1)
+    ms, md = describe(image), describe(edges)
+    _check(lib().b200cv_host_canny(ctypes.byref(ms), ctypes.byref(md), ctypes.c_double(threshold1), ctypes.c_double(threshold2), _int32(apertureSize),
+                                   int(bool(L2gradient))), "Canny")
+    return edges
+
+
+def _canny_derivs(dx, dy, threshold1, threshold2, edges=None, L2gradient=False):
+    import torch
+    from . import _canny_derivs as dev
+    out = dev(torch.from_numpy(np.ascontiguousarray(dx)).cuda(), torch.from_numpy(np.ascontiguousarray(dy)).cuda(), threshold1, threshold2,
+              None, L2gradient)
+    torch.cuda.synchronize()
+    res = out.cpu().numpy()
+    if edges is None:
+        return res
+    edges[...] = res
+    return edges
+
+
 def Scharr(src, ddepth, dx, dy, scale=1.0, delta=0.0, borderType=BORDER_DEFAULT, dst=None):
     return Sobel(src, ddepth, dx, dy, -1, scale, delta, borderType, dst)
 

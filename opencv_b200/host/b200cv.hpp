@@ -5,8 +5,8 @@
 //   b200cv::Filter + create*Filter               the cv::cuda::Filter shape used by samples/cpp/tutorial_code/gpu/gpu-basics-similarity
 //                                               (createGaussianFilter(type, type, ksize, sigma) -> apply(src, dst, stream))
 //   b200cv::GaussianBlur, sepFilter2D, filter2D, Sobel, resize, warpAffine, warpPerspective, cvtColor, matchTemplate, cornerHarris,
-//   cornerMinEigenVal, goodFeaturesToTrack      same argument order and meaning as imgproc.hpp:1544,1723,1702,1862,2422,2450,2482,3736,
-//                                               3916,1948,1921,2096, with a trailing Stream& like the cv::cuda:: functions
+//   cornerMinEigenVal, goodFeaturesToTrack,     same argument order and meaning as imgproc.hpp:1544,1723,1702,1862,2422,2450,2482,3736,
+//   Canny                                       3916,1948,1921,2096,1889,1907, with a trailing Stream& like the cv::cuda:: functions
 // With -DB200CV_WITH_OPENCV (OpenCV headers on the include path) b200cv_opencv.hpp adds namespace b200cv::cuda: the same operations over
 // cv::InputArray / cv::OutputArray (cv::Mat, cv::cuda::GpuMat, cv::cuda::HostMem) with cv::cuda's Filter / Stream& shapes.
 // Errors: the C ABI status is turned into b200cv::Error (std::runtime_error); NOT_IMPLEMENTED is b200cv::NotImplemented.
@@ -195,6 +195,13 @@ inline void cornerHarris(const GpuMat& src, GpuMat& dst, int blockSize, int ksiz
 { B200CV_DST(dst, src, makeType(CV_32F, 1)); b200cvMat a = src.desc(), b = dst.desc(); check(b200cv_corner_harris(&a, &b, blockSize, ksize, k, borderType, s.cudaPtr()), "cornerHarris"); }
 inline void cornerMinEigenVal(const GpuMat& src, GpuMat& dst, int blockSize, int ksize = 3, int borderType = BORDER_DEFAULT, Stream& s = Stream::Null())
 { B200CV_DST(dst, src, makeType(CV_32F, 1)); b200cvMat a = src.desc(), b = dst.desc(); check(b200cv_corner_min_eigen_val(&a, &b, blockSize, ksize, borderType, s.cudaPtr()), "cornerMinEigenVal"); }
+// cv::Canny (imgproc.hpp:1889, :1907): 8-bit image -> 8UC1 edges; or 16S derivatives dx, dy -> 8UC1 edges
+inline void Canny(const GpuMat& image, GpuMat& edges, double threshold1, double threshold2, int apertureSize = 3, bool L2gradient = false, Stream& s = Stream::Null())
+{ B200CV_DST(edges, image, makeType(CV_8U, 1)); b200cvMat a = image.desc(), b = edges.desc();
+  check(b200cv_canny(&a, &b, threshold1, threshold2, apertureSize, L2gradient ? 1 : 0, s.cudaPtr()), "Canny"); }
+inline void Canny(const GpuMat& dx, const GpuMat& dy, GpuMat& edges, double threshold1, double threshold2, bool L2gradient = false, Stream& s = Stream::Null())
+{ B200CV_DST(edges, dx, makeType(CV_8U, 1)); b200cvMat a = dx.desc(), b = dy.desc(), c = edges.desc();
+  check(b200cv_canny_derivs(&a, &b, &c, threshold1, threshold2, L2gradient ? 1 : 0, s.cudaPtr()), "Canny"); }
 inline void goodFeaturesToTrack(const GpuMat& image, std::vector<Point2f>& corners, int maxCorners, double qualityLevel, double minDistance, int blockSize = 3,
                                 int gradientSize = 3, bool useHarrisDetector = false, double k = 0.04, Stream& s = Stream::Null())
 { int cap = maxCorners > 0 ? maxCorners : image.rows * image.cols; std::vector<float> pts((size_t)2 * cap * image.frames); std::vector<int> cnt(image.frames);

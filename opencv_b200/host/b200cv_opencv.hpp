@@ -4,7 +4,7 @@
 //
 //   namespace b200cv::cuda   what a user of cv::cuda:: switches to (rename the namespace, keep the code): the reference signatures of
 //       GaussianBlur / sepFilter2D / filter2D / Sobel / resize / warpAffine / warpPerspective / cvtColor / matchTemplate / cornerHarris /
-//       cornerMinEigenVal / goodFeaturesToTrack (imgproc.hpp:1544,1723,1702,1862,2422,2450,2482,3736,3916,1948,1921,2096) + Stream&, and
+//       cornerMinEigenVal / goodFeaturesToTrack / Canny (imgproc.hpp:1544,1723,1702,1862,2422,2450,2482,3736,3916,1948,1921,2096,1889,1907) + Stream&, and
 //       GFTTDetector (features2d/src/gftt.cpp), createGaussianFilter / createSeparableLinearFilter / createLinearFilter / createSobelFilter -> Ptr<Filter>, Filter::apply(InputArray,
 //       OutputArray, Stream&) -- the usage of samples/cpp/tutorial_code/gpu/gpu-basics-similarity/gpu-basics-similarity.cpp:392-404.
 //   Array kinds accepted (core/include/opencv2/core/mat.hpp:163-188):
@@ -261,6 +261,32 @@ inline void cornerHarris(cv::InputArray src, cv::OutputArray dst, int blockSize,
 {
     Arr a = input(src, "cornerHarris"), b = output(dst, a.m.rows, a.m.cols, CV_32FC1, a.device, "cornerHarris");
     check(a.device ? b200cv_corner_harris(&a.m, &b.m, blockSize, ksize, k, borderType, s.cudaPtr()) : b200cv_host_corner_harris(&a.m, &b.m, blockSize, ksize, k, borderType), "cornerHarris");
+}
+inline void Canny(cv::InputArray image, cv::OutputArray edges, double threshold1, double threshold2, int apertureSize = 3, bool L2gradient = false,
+                  Stream& s = Stream::Null())
+{
+    Arr a = input(image, "Canny"), b = output(edges, a.m.rows, a.m.cols, CV_8UC1, a.device, "Canny");
+    const int l2 = L2gradient ? 1 : 0;
+    check(a.device ? b200cv_canny(&a.m, &b.m, threshold1, threshold2, apertureSize, l2, s.cudaPtr())
+                   : b200cv_host_canny(&a.m, &b.m, threshold1, threshold2, apertureSize, l2), "Canny");
+}
+// host derivatives are uploaded, the edges downloaded (there is no batched host path for this overload)
+inline void Canny(cv::InputArray dx, cv::InputArray dy, cv::OutputArray edges, double threshold1, double threshold2, bool L2gradient = false,
+                  Stream& s = Stream::Null())
+{
+    Arr a = input(dx, "Canny dx"), b = input(dy, "Canny dy");
+    if (a.device != b.device) throw Error(B200CV_ERR_BAD_ARG, "Canny: dx and dy must live on the same side");
+    const int l2 = L2gradient ? 1 : 0;
+    if (a.device) {
+        Arr e = output(edges, a.m.rows, a.m.cols, CV_8UC1, true, "Canny");
+        check(b200cv_canny_derivs(&a.m, &b.m, &e.m, threshold1, threshold2, l2, s.cudaPtr()), "Canny");
+        return;
+    }
+    DeviceMat ux, uy, ue(a.m.rows, a.m.cols, CV_8UC1);
+    ux.upload(dx, s); uy.upload(dy, s);
+    Arr da = input(ux, "Canny dx"), db = input(uy, "Canny dy"), de = input(ue, "Canny edges");
+    check(b200cv_canny_derivs(&da.m, &db.m, &de.m, threshold1, threshold2, l2, s.cudaPtr()), "Canny");
+    ue.download(edges, s);
 }
 inline void cornerMinEigenVal(cv::InputArray src, cv::OutputArray dst, int blockSize, int ksize = 3, int borderType = cv::BORDER_DEFAULT, Stream& s = Stream::Null())
 {
