@@ -7,6 +7,10 @@
 //            (anti)symmetric taps goes centre-out: fma(x0, k0, (x-1 + x1) k1), then fma(x-2 + x2, k2, .) (SymmRowSmallVec_32f :1768-1844)
 //   columns  mirrored rows first: s = fma(ky[c], S[c], delta); s = fma(ky[c+k], S[c+k] +/- S[c-k], s)  (SymmColumnVec_32f :1878-1949,
 //            SymmColumnVec_32f8u :1158-1202).  Kernels that are not (anti)symmetric are left to the generic kernel.
+//   Taps are centred in a zero-padded bucket of KB.  Float sources whose kernel has zero taps the reference never evaluates -- the
+//   padding to the bucket (px / py), the centre of an antisymmetric column kernel or of antisymmetric 3/5-tap rows -- run an
+//   instantiation (SKIP0) that skips them: fma(inf, 0, s) would be NaN where the reference has a finite value or an infinity.  Full
+//   symmetric buckets keep the unpredicated loops; 8-bit rows are finite, so they need no such instantiation.
 // Same arithmetic as sep_fast_kernel<.,.,M_FLOAT,KB> in sepfilter.cu -- only the data movement differs: ONE thread issues a 3-D cp.async.bulk.tensor box load of the
 // (192+2r) x (32+2r) float tile into shared memory and the CTA waits on an mbarrier, so the loads of one CTA overlap the
 // arithmetic of the other CTAs resident on the SM instead of stalling every thread on its own LDG (the generic kernel was
@@ -29,12 +33,13 @@ struct SF32Params {
     int has_dog;
     int row_small;             // float source, 3/5 (anti)symmetric taps: 1 symmetric, 2 antisymmetric (centre-out order), 0 tap order
     unsigned col_sign;         // 0: symmetric column kernel, 0x80000000: antisymmetric (S[c+k] - S[c-k])
+    int px, py;                // zero taps padding kx / ky to KB on each side: skipped (SKIP0), so a non-finite pixel reaches only the real footprint
     int nch;                   // chunks of SF_TH output rows one CTA walks down (1 = the plain tile kernel)
 };
 
 // ---- up to 11 taps: the plain tile kernel (one 192 x 32 tile per CTA, 3 CTAs per SM at 80 registers) -- the walking kernel below carries
 //      state that does not fit that register budget (its tile form is slower at 3 and 9 taps) ----
-template <int KB, typename ST, typename DT>
+template <int KB, typename ST, typename DT, bool SKIP0>
 __global__ void __launch_bounds__(256, 3) sep_f32_tile_kernel(const __grid_constant__ CUtensorMap tmap, Img dst, const __grid_constant__ SF32Params p)
 {
     constexpr int RB = KB / 2;
@@ -112,10 +117,10 @@ __global__ void __launch_bounds__(256, 3) sep_f32_tile_kernel(const __grid_const
 #pragma unroll
                     for (int o = 0; o < NO; o++) {
                         const float* x = win + OFF + o + RB;      // centre tap
-                        // symmetric: fma(x0, k0, (x-1 + x1) k1); antisymmetric: (x1 - x-1) k1  (k0 = 0: fma(x0, 0, t) = t)
+                        // symmetric: fma(x0, k0, (x-1 + x1) k1); antisymmetric: (x1 - x-1) k1, no centre term (SKIP0; fma(x0, 0, t) = t for finite x0)
                         float t = __fmul_rn(__fadd_rn(x[1], __uint_as_float(__float_as_uint(x[-1]) ^ sg)), p.kx[RB + 1]);
-                        t = fmaf(x[0], p.kx[RB], t);
-                        if constexpr (KB == 5) t = fmaf(__fadd_rn(x[2], __uint_as_float(__float_as_uint(x[-2]) ^ sg)), p.kx[RB + 2], t);
+                        if (!SKIP0 || p.row_small != 2) t = fmaf(x[0], p.kx[RB], t);
+                        if constexpr (KB == 5) if (!SKIP0 || !p.px) t = fmaf(__fadd_rn(x[2], __uint_as_float(__float_as_uint(x[-2]) ^ sg)), p.kx[RB + 2], t);
                         acc[o] = t;
                     }
                     done = true;
@@ -126,7 +131,8 @@ __global__ void __launch_bounds__(256, 3) sep_f32_tile_kernel(const __grid_const
                 for (int o = 0; o < NO; o++) {
                     float t = 0.f;
 #pragma unroll
-                    for (int i = 0; i < KB; i++) t = fmaf(win[OFF + o + i], p.kx[i], t);
+                    for (int i = 0; i < KB; i++)
+                        if (!SKIP0 || (i >= p.px && i < KB - p.px)) t = fmaf(win[OFF + o + i], p.kx[i], t);
                     acc[o] = t;
                 }
             }
@@ -167,10 +173,11 @@ __global__ void __launch_bounds__(256, 3) sep_f32_tile_kernel(const __grid_const
                 float acc[CW];
 #pragma unroll
                 for (int c = 0; c < CW; c++) {
-                    float t = fmaf(p.ky[RB], win[o + RB][c], p.delta);
+                    float t = (SKIP0 && p.col_sign) ? p.delta : fmaf(p.ky[RB], win[o + RB][c], p.delta);   // antisymmetric: no centre row
 #pragma unroll
                     for (int k = 1; k <= RB; k++)
-                        t = fmaf(p.ky[RB + k], __fadd_rn(win[o + RB + k][c], __uint_as_float(__float_as_uint(win[o + RB - k][c]) ^ p.col_sign)), t);
+                        if (!SKIP0 || k <= RB - p.py)
+                            t = fmaf(p.ky[RB + k], __fadd_rn(win[o + RB + k][c], __uint_as_float(__float_as_uint(win[o + RB - k][c]) ^ p.col_sign)), t);
                     acc[c] = t;
                 }
                 if constexpr (sizeof(DT) == 1) {
@@ -213,12 +220,12 @@ __global__ void __launch_bounds__(256, 3) sep_f32_tile_kernel(const __grid_const
     }
 }
 
-template <int KB, typename ST, typename DT>
+template <int KB, typename ST, typename DT, bool SKIP0>
 static int launch_sf32_tile(const CUtensorMap& tm, const Img& d, const SF32Params& p, int frames, cudaStream_t st)
 {
     constexpr int IH = SF_TH + KB - 1;
     const size_t smem = (((size_t)IH * SF_IW * sizeof(ST) + 127) & ~(size_t)127) + (size_t)IH * SF_TW * sizeof(float);
-    auto kern = sep_f32_tile_kernel<KB, ST, DT>;
+    auto kern = sep_f32_tile_kernel<KB, ST, DT, SKIP0>;
     static PerDeviceFlag attr_pd; bool& attr = attr_pd.cur();
     if (!attr) { B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = true; }
     dim3 grid(div_up((unsigned)p.W, SF_TW), div_up((unsigned)p.H, SF_TH), (unsigned)frames);
@@ -236,7 +243,7 @@ static int launch_sf32_tile(const CUtensorMap& tm, const Img& d, const SF32Param
 // (1.9x the row-pass work at 27 taps).  The next chunk's TMA load is issued
 // right after the row pass and lands during the column pass.  Rows above / below the image (mirroring borders): the row filter commutes
 // with the vertical mirror, so those filtered rows are copies of the mirrored rows' filtered rows.
-template <int KB, typename ST, typename DT>
+template <int KB, typename ST, typename DT, bool SKIP0>
 __global__ void __launch_bounds__(256, (KB <= 11 ? 3 : 2)) sep_f32_tma_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap tmap_tail, Img src, Img dst,
                                                                               const __grid_constant__ SF32Params p)
 {
@@ -319,10 +326,10 @@ __global__ void __launch_bounds__(256, (KB <= 11 ? 3 : 2)) sep_f32_tma_kernel(co
 #pragma unroll
                     for (int o = 0; o < NO; o++) {
                         const float* x = win + OFF + o + RB;      // centre tap
-                        // symmetric: fma(x0, k0, (x-1 + x1) k1); antisymmetric: (x1 - x-1) k1  (k0 = 0: fma(x0, 0, t) = t)
+                        // symmetric: fma(x0, k0, (x-1 + x1) k1); antisymmetric: (x1 - x-1) k1, no centre term (SKIP0; fma(x0, 0, t) = t for finite x0)
                         float t = __fmul_rn(__fadd_rn(x[1], __uint_as_float(__float_as_uint(x[-1]) ^ sg)), p.kx[RB + 1]);
-                        t = fmaf(x[0], p.kx[RB], t);
-                        if constexpr (KB == 5) t = fmaf(__fadd_rn(x[2], __uint_as_float(__float_as_uint(x[-2]) ^ sg)), p.kx[RB + 2], t);
+                        if (!SKIP0 || p.row_small != 2) t = fmaf(x[0], p.kx[RB], t);
+                        if constexpr (KB == 5) if (!SKIP0 || !p.px) t = fmaf(__fadd_rn(x[2], __uint_as_float(__float_as_uint(x[-2]) ^ sg)), p.kx[RB + 2], t);
                         acc[o] = t;
                     }
                     done = true;
@@ -333,7 +340,8 @@ __global__ void __launch_bounds__(256, (KB <= 11 ? 3 : 2)) sep_f32_tma_kernel(co
                 for (int o = 0; o < NO; o++) {
                     float t = 0.f;
 #pragma unroll
-                    for (int i = 0; i < KB; i++) t = fmaf(win[OFF + o + i], p.kx[i], t);
+                    for (int i = 0; i < KB; i++)
+                        if (!SKIP0 || (i >= p.px && i < KB - p.px)) t = fmaf(win[OFF + o + i], p.kx[i], t);
                     acc[o] = t;
                 }
             }
@@ -417,10 +425,11 @@ __global__ void __launch_bounds__(256, (KB <= 11 ? 3 : 2)) sep_f32_tma_kernel(co
                 float acc[CW];
 #pragma unroll
                 for (int c = 0; c < CW; c++) {
-                    float t = fmaf(p.ky[RB], win[o + RB][c], p.delta);
+                    float t = (SKIP0 && p.col_sign) ? p.delta : fmaf(p.ky[RB], win[o + RB][c], p.delta);   // antisymmetric: no centre row
 #pragma unroll
                     for (int k = 1; k <= RB; k++)
-                        t = fmaf(p.ky[RB + k], __fadd_rn(win[o + RB + k][c], __uint_as_float(__float_as_uint(win[o + RB - k][c]) ^ p.col_sign)), t);
+                        if (!SKIP0 || k <= RB - p.py)
+                            t = fmaf(p.ky[RB + k], __fadd_rn(win[o + RB + k][c], __uint_as_float(__float_as_uint(win[o + RB - k][c]) ^ p.col_sign)), t);
                     acc[c] = t;
                 }
                 if constexpr (sizeof(DT) == 1) {
@@ -464,7 +473,7 @@ __global__ void __launch_bounds__(256, (KB <= 11 ? 3 : 2)) sep_f32_tma_kernel(co
   }
 }
 
-template <int KB, typename ST, typename DT>
+template <int KB, typename ST, typename DT, bool SKIP0>
 static int launch_sf32(const CUtensorMap& tm, const CUtensorMap& tm_tail, const Img& s, const Img& d, SF32Params& p, int frames, cudaStream_t st)
 {
     constexpr int IH = SF_TH + KB - 1;
@@ -473,7 +482,7 @@ static int launch_sf32(const CUtensorMap& tm, const CUtensorMap& tm_tail, const 
     const long tiles = (long)div_up((unsigned)p.W, SF_TW) * div_up((unsigned)p.H, SF_TH) * frames;
     p.nch = (KB >= 13 && tiles >= 8L * 2 * num_sms()) ? 4 : (KB >= 13 && tiles >= 4L * 2 * num_sms()) ? 2 : 1;
     if (p.has_dog && getenv("B200CV_SEP_DOG_TILE")) p.nch = 1;      // measurement switch: the plain tile kernel for the fused-DoG blurs
-    auto kern = sep_f32_tma_kernel<KB, ST, DT>;
+    auto kern = sep_f32_tma_kernel<KB, ST, DT, SKIP0>;
     static PerDeviceFlag attr_pd; bool& attr = attr_pd.cur();
     if (!attr) { B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = true; }
     dim3 grid(div_up((unsigned)p.W, SF_TW), div_up((unsigned)p.H, (unsigned)(SF_TH * p.nch)), (unsigned)frames);
@@ -491,6 +500,9 @@ static int symmetry_of(const float* k, int n)
     for (int i = 0; i < n; i++) { if (k[i] != k[n - 1 - i]) sy = false; if (k[i] != -k[n - 1 - i]) as = false; }
     return sy ? 1 : as ? 2 : 0;
 }
+
+template <typename ST, typename DT, bool SKIP0>
+static int launch_kb(int KB, const CUtensorMap& tm, const CUtensorMap& tm_tail, const Img& s, const Img& d, SF32Params& p, cudaStream_t st);
 
 template <typename ST, typename DT>
 static int sep_float_fast(const Img& s, const Img& d, const float* kx, int nx, const float* ky, int ny, float delta, int border, const Img* dog, cudaStream_t st)
@@ -511,25 +523,33 @@ static int sep_float_fast(const Img& s, const Img& d, const float* kx, int nx, c
     for (int i = 0; i < ny; i++) p.ky[(KB - ny) / 2 + i] = ky[i];
     p.delta = delta; p.W = s.cols; p.H = s.rows; p.border = border;
     p.row_small = rsym; p.col_sign = csym == 2 ? 0x80000000u : 0u;
+    p.px = (KB - nx) / 2; p.py = (KB - ny) / 2;
     if (dog) { p.dog = *dog; p.has_dog = 1; }
     CUtensorMap tm, tm_tail;
     const bool march = KB >= 13;
     int rc = make_tensor_map_3d(&tm, s.data, (int)sizeof(ST), s.cols, s.rows, s.frames, s.step, s.fstep, SF_IW, march ? SF_TH : SF_TH + KB - 1);
     if (rc) return rc;
     if ((rc = make_tensor_map_3d(&tm_tail, s.data, (int)sizeof(ST), s.cols, s.rows, s.frames, s.step, s.fstep, SF_IW, KB - 1))) return rc;
+    if (sizeof(ST) == 4 && (p.px || p.py || rsym == 2 || csym == 2)) return launch_kb<ST, DT, true>(KB, tm, tm_tail, s, d, p, st);
+    return launch_kb<ST, DT, false>(KB, tm, tm_tail, s, d, p, st);
+}
+
+template <typename ST, typename DT, bool SKIP0>
+static int launch_kb(int KB, const CUtensorMap& tm, const CUtensorMap& tm_tail, const Img& s, const Img& d, SF32Params& p, cudaStream_t st)
+{
     switch (KB) {
-    case 3: return launch_sf32_tile<3, ST, DT>(tm, d, p, s.frames, st);
-    case 5: return launch_sf32_tile<5, ST, DT>(tm, d, p, s.frames, st);
-    case 7: return launch_sf32_tile<7, ST, DT>(tm, d, p, s.frames, st);
-    case 9: return launch_sf32_tile<9, ST, DT>(tm, d, p, s.frames, st);
-    case 11: return launch_sf32_tile<11, ST, DT>(tm, d, p, s.frames, st);
-    case 13: return launch_sf32<13, ST, DT>(tm, tm_tail, s, d, p, s.frames, st);
-    case 15: return launch_sf32<15, ST, DT>(tm, tm_tail, s, d, p, s.frames, st);
-    case 17: return launch_sf32<17, ST, DT>(tm, tm_tail, s, d, p, s.frames, st);
-    case 21: return launch_sf32<21, ST, DT>(tm, tm_tail, s, d, p, s.frames, st);
-    case 25: return launch_sf32<25, ST, DT>(tm, tm_tail, s, d, p, s.frames, st);
-    case 27: return launch_sf32<27, ST, DT>(tm, tm_tail, s, d, p, s.frames, st);
-    case 31: return launch_sf32<31, ST, DT>(tm, tm_tail, s, d, p, s.frames, st);
+    case 3: return launch_sf32_tile<3, ST, DT, SKIP0>(tm, d, p, s.frames, st);
+    case 5: return launch_sf32_tile<5, ST, DT, SKIP0>(tm, d, p, s.frames, st);
+    case 7: return launch_sf32_tile<7, ST, DT, SKIP0>(tm, d, p, s.frames, st);
+    case 9: return launch_sf32_tile<9, ST, DT, SKIP0>(tm, d, p, s.frames, st);
+    case 11: return launch_sf32_tile<11, ST, DT, SKIP0>(tm, d, p, s.frames, st);
+    case 13: return launch_sf32<13, ST, DT, SKIP0>(tm, tm_tail, s, d, p, s.frames, st);
+    case 15: return launch_sf32<15, ST, DT, SKIP0>(tm, tm_tail, s, d, p, s.frames, st);
+    case 17: return launch_sf32<17, ST, DT, SKIP0>(tm, tm_tail, s, d, p, s.frames, st);
+    case 21: return launch_sf32<21, ST, DT, SKIP0>(tm, tm_tail, s, d, p, s.frames, st);
+    case 25: return launch_sf32<25, ST, DT, SKIP0>(tm, tm_tail, s, d, p, s.frames, st);
+    case 27: return launch_sf32<27, ST, DT, SKIP0>(tm, tm_tail, s, d, p, s.frames, st);
+    case 31: return launch_sf32<31, ST, DT, SKIP0>(tm, tm_tail, s, d, p, s.frames, st);
     }
     return B200CV_NOT_IMPLEMENTED;
 }

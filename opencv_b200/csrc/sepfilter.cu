@@ -17,7 +17,9 @@
 //
 // Two kernels:
 //  * sep_fast_kernel<ST,DT,MODE,KB>  single-channel images, odd centred kernels up to 31 taps; tap count is a
-//      template bucket so the taps are constant-bank operands and all window indexing is resolved at compile time;
+//      template bucket so the taps are constant-bank operands and all window indexing is resolved at compile time; for a
+//      float source the zero taps the reference never evaluates (the padding to the bucket, the centre of antisymmetric columns and
+//      3/5-tap rows) are skipped (SKIP0, here and in the generic kernel), so a non-finite pixel reaches only the real footprint;
 //  * sep_generic_kernel<ST,DT,MODE>  any channel count / anchor / tap count <= 33, run-time loops.
 #include <cmath>
 #include <vector>
@@ -43,6 +45,7 @@ struct SepParams {
     int even_limit;   // M_FIXED16: row elements < even_limit round half-to-even (sepFilter2D's vector body), the rest half-up
     int row_small;    // M_FLOAT, float source, 3/5 (anti)symmetric taps: 1|2 = centre-out order of SymmRowSmallVec_32f, 0 = tap order
     int col_mode;     // M_FLOAT: 1|2 = (anti)symmetric column kernel, mirrored rows added first; 0 = scalar ColumnFilter order (no FMA)
+    int px, py;       // M_FLOAT fast kernel: zero taps padding kx / ky to the bucket on each side, not evaluated under SKIP0 (fma(inf, 0, s) = NaN)
 };
 
 template <typename T> __device__ __forceinline__ float to_f(T v) { return (float)v; }
@@ -107,7 +110,7 @@ __global__ void __launch_bounds__(256) sep_generic_kernel(Img src, Img dst, SepP
             const int m = nx / 2;
             const float sg = p.row_small == 2 ? -1.f : 1.f;
             acc = __fmul_rn(__fadd_rn(s[(m + 1) * cn], sg * s[(m - 1) * cn]), p.t.kx[m + 1]);
-            acc = fmaf(s[m * cn], p.t.kx[m], acc);
+            if (p.row_small != 2) acc = fmaf(s[m * cn], p.t.kx[m], acc);      // antisymmetric: no centre term
             if (nx == 5) acc = fmaf(__fadd_rn(s[(m + 2) * cn], sg * s[(m - 2) * cn]), p.t.kx[m + 2], acc);
         } else {
             for (int i = 0; i < nx; i++) acc = fmaf(s[i * cn], p.t.kx[i], acc);
@@ -126,7 +129,7 @@ __global__ void __launch_bounds__(256) sep_generic_kernel(Img src, Img dst, SepP
             if (p.col_mode) {                             // SymmColumnVec_32f / _32f8u: filter.simd.hpp:1878-1949, :1158-1202
                 const int c = ny / 2;
                 const float sg = p.col_mode == 2 ? -1.f : 1.f;
-                acc = fmaf(p.t.ky[c], s[c * mid_w], p.delta);
+                acc = p.col_mode == 2 ? p.delta : fmaf(p.t.ky[c], s[c * mid_w], p.delta);      // antisymmetric: no centre row
                 for (int k = 1; k <= c; k++) acc = fmaf(p.t.ky[c + k], __fadd_rn(s[(c + k) * mid_w], sg * s[(c - k) * mid_w]), acc);
             } else {                                      // scalar ColumnFilter: products rounded before they are added, :2590-2640
                 acc = fmaf(s[0], p.t.ky[0], p.delta);      // only the delta term is contracted in the reference object
@@ -158,7 +161,7 @@ __device__ __forceinline__ float byte_to_float(uint32_t w, int j)
     return __uint_as_float(__byte_perm(w, 0x4B000000u, 0x7540u | (unsigned)j)) - 8388608.0f;
 }
 
-template <typename ST, typename DT, int MODE, int KB>
+template <typename ST, typename DT, int MODE, int KB, bool SKIP0>
 __global__ void __launch_bounds__(256) sep_fast_kernel(Img src, Img dst, const __grid_constant__ SepParams p, int TH)
 {
     constexpr int RB = KB / 2;
@@ -234,8 +237,8 @@ __global__ void __launch_bounds__(256) sep_fast_kernel(Img src, Img dst, const _
 #pragma unroll
                 for (int o = 0; o < F_R; o++) {
                     float t = __fmul_rn(__fadd_rn((float)x[o + 1], sg * (float)x[o - 1]), p.t.kx[RB + 1]);
-                    t = fmaf((float)x[o], p.t.kx[RB], t);
-                    if (KB == 5) t = fmaf(__fadd_rn((float)x[o + 2], sg * (float)x[o - 2]), p.t.kx[RB + 2], t);
+                    if (!SKIP0 || p.row_small != 2) t = fmaf((float)x[o], p.t.kx[RB], t);
+                    if (KB == 5 && (!SKIP0 || !p.px)) t = fmaf(__fadd_rn((float)x[o + 2], sg * (float)x[o - 2]), p.t.kx[RB + 2], t);
                     acc[o] = t;
                 }
             } else {
@@ -252,7 +255,7 @@ __global__ void __launch_bounds__(256) sep_fast_kernel(Img src, Img dst, const _
 #pragma unroll
                             for (int o = 0; o < F_R; o++) {
                                 const int i = e - o;
-                                if (i >= 0 && i < KB) acc[o] = fmaf(vals[b], p.t.kx[i], acc[o]);
+                                if (i >= 0 && i < KB && (!SKIP0 || (i >= p.px && i < KB - p.px))) acc[o] = fmaf(vals[b], p.t.kx[i], acc[o]);
                             }
                         }
                     }
@@ -286,9 +289,13 @@ __global__ void __launch_bounds__(256) sep_fast_kernel(Img src, Img dst, const _
                     const float* ctr = mbase + (o + RB) * F_TW;
                     const float4 v0 = *(const float4*)ctr;
                     const float t0 = p.t.ky[RB];
-                    float a0 = fmaf(t0, v0.x, p.delta), a1 = fmaf(t0, v0.y, p.delta), a2 = fmaf(t0, v0.z, p.delta), a3 = fmaf(t0, v0.w, p.delta);
+                    float a0 = p.delta, a1 = p.delta, a2 = p.delta, a3 = p.delta;
+                    if (!SKIP0 || p.col_mode != 2) {                // antisymmetric: no centre row
+                        a0 = fmaf(t0, v0.x, p.delta); a1 = fmaf(t0, v0.y, p.delta); a2 = fmaf(t0, v0.z, p.delta); a3 = fmaf(t0, v0.w, p.delta);
+                    }
 #pragma unroll
                     for (int k = 1; k <= RB; k++) {
+                        if (SKIP0 && k > RB - p.py) break;          // zero taps padding ky to the bucket
                         const float4 va = *(const float4*)(ctr + k * F_TW), vb = *(const float4*)(ctr - k * F_TW);
                         const float t = p.t.ky[RB + k];
                         a0 = fmaf(t, __fadd_rn(va.x, sg * vb.x), a0); a1 = fmaf(t, __fadd_rn(va.y, sg * vb.y), a1);
@@ -346,7 +353,7 @@ __global__ void __launch_bounds__(256) sep_fast_kernel(Img src, Img dst, const _
 // ================================================================================================================
 // host dispatch
 // ================================================================================================================
-template <typename ST, typename DT, int MODE, int KB>
+template <typename ST, typename DT, int MODE, int KB, bool SKIP0>
 static int launch_fast(const Img& s, const Img& d, const SepParams& p, cudaStream_t st)
 {
     constexpr int RB = KB / 2;
@@ -358,7 +365,7 @@ static int launch_fast(const Img& s, const Img& d, const SepParams& p, cudaStrea
     if (s.rows <= 16) TH = 16;
     if (s.rows <= 8) TH = 8;
     size_t smem = smem_for(TH);
-    auto kern = sep_fast_kernel<ST, DT, MODE, KB>;
+    auto kern = sep_fast_kernel<ST, DT, MODE, KB, SKIP0>;
     static PerDeviceFlag attr_done_pd; bool& attr_done = attr_done_pd.cur();
     if (!attr_done) {
         B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
@@ -370,25 +377,34 @@ static int launch_fast(const Img& s, const Img& d, const SepParams& p, cudaStrea
     return B200CV_OK;
 }
 
-template <typename ST, typename DT, int MODE>
-static int launch_fast_k(int kb, const Img& s, const Img& d, const SepParams& p, cudaStream_t st)
+template <typename ST, typename DT, int MODE, bool SKIP0>
+static int launch_fast_kb(int kb, const Img& s, const Img& d, const SepParams& p, cudaStream_t st)
 {
     switch (kb) {
-    case 3: return launch_fast<ST, DT, MODE, 3>(s, d, p, st);
-    case 5: return launch_fast<ST, DT, MODE, 5>(s, d, p, st);
-    case 7: return launch_fast<ST, DT, MODE, 7>(s, d, p, st);
-    case 9: return launch_fast<ST, DT, MODE, 9>(s, d, p, st);
-    case 11: return launch_fast<ST, DT, MODE, 11>(s, d, p, st);
-    case 13: return launch_fast<ST, DT, MODE, 13>(s, d, p, st);
-    case 15: return launch_fast<ST, DT, MODE, 15>(s, d, p, st);
-    case 17: return launch_fast<ST, DT, MODE, 17>(s, d, p, st);
-    case 21: return launch_fast<ST, DT, MODE, 21>(s, d, p, st);
-    case 25: return launch_fast<ST, DT, MODE, 25>(s, d, p, st);
-    case 27: return launch_fast<ST, DT, MODE, 27>(s, d, p, st);
-    case 31: return launch_fast<ST, DT, MODE, 31>(s, d, p, st);
+    case 3: return launch_fast<ST, DT, MODE, 3, SKIP0>(s, d, p, st);
+    case 5: return launch_fast<ST, DT, MODE, 5, SKIP0>(s, d, p, st);
+    case 7: return launch_fast<ST, DT, MODE, 7, SKIP0>(s, d, p, st);
+    case 9: return launch_fast<ST, DT, MODE, 9, SKIP0>(s, d, p, st);
+    case 11: return launch_fast<ST, DT, MODE, 11, SKIP0>(s, d, p, st);
+    case 13: return launch_fast<ST, DT, MODE, 13, SKIP0>(s, d, p, st);
+    case 15: return launch_fast<ST, DT, MODE, 15, SKIP0>(s, d, p, st);
+    case 17: return launch_fast<ST, DT, MODE, 17, SKIP0>(s, d, p, st);
+    case 21: return launch_fast<ST, DT, MODE, 21, SKIP0>(s, d, p, st);
+    case 25: return launch_fast<ST, DT, MODE, 25, SKIP0>(s, d, p, st);
+    case 27: return launch_fast<ST, DT, MODE, 27, SKIP0>(s, d, p, st);
+    case 31: return launch_fast<ST, DT, MODE, 31, SKIP0>(s, d, p, st);
     }
     set_error("internal: no fast bucket for %d taps", kb);
     return B200CV_ERR_BAD_ARG;
+}
+
+// float sources with zero taps the reference never evaluates (padding to the bucket, antisymmetric centres): the instantiation that skips
+// them (8-bit rows and integer modes are finite)
+template <typename ST, typename DT, int MODE>
+static int launch_fast_k(int kb, const Img& s, const Img& d, const SepParams& p, cudaStream_t st)
+{
+    if (MODE == M_FLOAT && sizeof(ST) == 4 && (p.px || p.py || p.row_small == 2 || p.col_mode == 2)) return launch_fast_kb<ST, DT, MODE, true>(kb, s, d, p, st);
+    return launch_fast_kb<ST, DT, MODE, false>(kb, s, d, p, st);
 }
 
 static int fast_bucket(int k)
@@ -444,6 +460,7 @@ static int sep_dispatch(const Img& s, const Img& d, int cn, const float* kx, int
         for (int i = 0; i < nx; i++) p.t.kx[ox + i] = kx[i];
         for (int i = 0; i < ny; i++) p.t.ky[oy + i] = ky[i];
         p.t.nx = p.t.ny = kb; p.t.ax = p.t.ay = kb / 2;
+        p.px = ox; p.py = oy;
         return launch_fast_k<ST, DT, MODE>(kb, s, d, p, st);
     }
     if (nx > 33 || ny > 33) return B200CV_NOT_IMPLEMENTED;

@@ -15,7 +15,9 @@ Bars
                           exact in test_gpu_corner_exact.py
   SIFT pyramid .......... per level |d| <= 1e-3 absolute on a 0..255 scale (a chain of up to 5 f32 blurs per octave and 10 octaves;
                           NOTE the reference has no test that pins these pyramids -- the oracle is the reference's own code
-                          (oracle/_ref) or the same composition of public calls in the port)
+                          (oracle/_ref) or the same composition of public calls in the port).  Past the first octave whose width
+                          is not a multiple of 8 the reference's scalar tails set the bar; tests/test_gpu_sep_float_exact.py holds
+                          every level of every octave (and the whole pyramid) to the C port bit for bit
 """
 import numpy as np
 import pytest

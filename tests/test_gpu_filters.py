@@ -5,7 +5,9 @@ Tolerances
   f32 GaussianBlur / sepFilter2D, and 8-bit sepFilter2D through float: BIT-EXACT wherever the reference runs a full SIMD vector
     (same operation order: centre-out small rows, mirrored-pair columns, FMA); the last W*cn mod 8 (float source) / mod 32 (8-bit
     source) elements of each row are the reference's scalar remainder loops: |d| <= 1e-4 + 1e-5 |ref| there (the reference's own
-    bar for the whole image: test_filter.cpp:826-830 uses 1e-5 relative)
+    bar for the whole image: test_filter.cpp:826-830 uses 1e-5 relative).  These bars describe the reference's scalar tails, not
+    the kernels: tests/test_gpu_sep_float_exact.py holds every float separable kernel to the C port bit for bit over the whole
+    destination (remainder columns, anchors, walked chunks, 8-bit rounding, non-finite pixels)
   filter2D u8: BIT-EXACT below 130 taps (the CPU's direct float sum, reproduced in operation order); <= 1 LSB from 130 taps on, where
     the CPU uses a DFT (its own test allows 2, test_filter.cpp:420-425) and the GPU an exact fixed-point tensor-core correlation.
     Against the reference these bars stay; tests/test_gpu_filter2d_tc_exact.py holds both tensor-core kernels (8-bit: bit for bit;
