@@ -859,9 +859,9 @@ __global__ void __launch_bounds__(256) remap_kernel(Img src, Img dst, Img m1, Im
     if (kind == MAP_FIXED) {
         const short* xy = m1.row<short>(0, y) + 2 * x;
         const int fr = m2.data ? (m2.row<unsigned short>(0, y)[x] & 1023) : 0;
-        if (INTERP == W_NN) {       // NNDeltaTab_i as the reference fills it: +1 where the 5-bit fraction is BELOW 1/2 (:237-238, :1176-1181)
+        if (INTERP == W_NN && m2.data) {       // NNDeltaTab_i as the reference fills it: +1 where the 5-bit fraction is BELOW 1/2 (:237-238, :1176-1181)
             sx = (short)(xy[0] + ((fr & 31) < 16)); sy = (short)(xy[1] + ((fr >> 5) < 16));
-        } else { sx = xy[0]; sy = xy[1]; a = fr; }
+        } else { sx = xy[0]; sy = xy[1]; a = fr; }      // NEAREST without a fraction map: the coordinates as they are (:1166)
     } else {
         float mx, my;
         if (kind == MAP_PLANAR_F32) { mx = m1.row<float>(0, y)[x]; my = m2.row<float>(0, y)[x]; }

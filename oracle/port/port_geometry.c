@@ -384,8 +384,10 @@ static void map_coords(const PortMaps* mp, int x, int y, int interp, int* sx, in
         const short* xy = (const short*)((const char*)mp->m1 + (size_t)y * mp->s1) + 2 * x;
         int fr = mp->m2 ? (((const unsigned short*)((const char*)mp->m2 + (size_t)y * mp->s2))[x] & 1023) : 0;
         /* NNDeltaTab_i is filled as (fraction < 1/2) (imgwarp.cpp:237-238) -- and only once a bilinear table has been built in the process;
-           before that it is all zeros.  The table as built is what is reproduced here. */
-        if (interp == 0) { *sx = (short)(xy[0] + ((fr & 31) < 16)); *sy = (short)(xy[1] + ((fr >> 5) < 16)); }
+           before that it is all zeros.  The table as built is what is reproduced here.  Without a fraction map the coordinates are
+           "already in the right format" (:1166) and the table is not consulted. */
+        if (interp == 0 && !mp->m2) { *sx = xy[0]; *sy = xy[1]; }
+        else if (interp == 0) { *sx = (short)(xy[0] + ((fr & 31) < 16)); *sy = (short)(xy[1] + ((fr >> 5) < 16)); }
         else { *sx = xy[0]; *sy = xy[1]; *a = fr; }
         return;
     }

@@ -5,6 +5,10 @@ Bars (the reference's own strict test allows |d| <= 1 for LINEAR/CUBIC, test_img
                                                              reference's u8 CUBIC column pass is reproduced)
   warp* u8 (NEAREST/LINEAR/CUBIC) .......................... BIT-EXACT (fixed-point coordinates + 2^15 tap tables)
   f32 (resize and warps, every interpolation and border) ... BIT-EXACT: same float operations in the same order
+
+The warps here run at a few everyday geometries and at 8K.  tests/test_gpu_warp_exact.py takes each of the four warp kernels to its
+tile, column-block, footprint and alignment edges (table: tests/warp_cases.py; the port it compares with is held to the reference
+over the same table by tests/test_warp_port.py).
 """
 import numpy as np
 import pytest
