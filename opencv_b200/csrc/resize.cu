@@ -248,9 +248,9 @@ __global__ void __launch_bounds__(256) resize_area2_f32_kernel(Img src, Img dst,
     for (int c = 0; c < CN; c++) {
         float a = s0[c], b = s0[c + CN], e = s1[c], g = s1[c + CN];
         // 1 / 4 channels: the 4-lane SIMD body adds row sums, (a+b)+(e+g); 3 channels and the single-channel remainder columns
-        // (dw % 4, resize.cpp:3012-3024) run the scalar loop, ((a+b)+e)+g
+        // (dw % 4, resize.cpp:3012-3024) run the scalar loop, 0 + (((a+b)+e)+g) -- its sum starts at +0, so -0 comes out as +0
         const bool seq = CN == 3 || (CN == 1 && x >= (dw & ~3));
-        float sum = seq ? __fadd_rn(__fadd_rn(__fadd_rn(a, b), e), g) : __fadd_rn(__fadd_rn(a, b), __fadd_rn(e, g));
+        float sum = seq ? __fadd_rn(0.f, __fadd_rn(__fadd_rn(__fadd_rn(a, b), e), g)) : __fadd_rn(__fadd_rn(a, b), __fadd_rn(e, g));
         d[c] = __fmul_rn(sum, 0.25f);
     }
 }

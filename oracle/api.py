@@ -154,7 +154,7 @@ class Oracle:
         return dst
 
     def resize_fxfy(self, src, fx, fy, interpolation=1):
-        """cv::resize(src, dst, Size(), fx, fy): only the real reference has it"""
+        """cv::resize(src, dst, Size(), fx, fy); the port has NEAREST / LINEAR / CUBIC and the 2 x 2 decimation on even sizes"""
         src = np.ascontiguousarray(src)
         sh, sw = src.shape[:2]
         dw, dh = int(round(sw * fx)), int(round(sh * fy))

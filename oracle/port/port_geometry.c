@@ -44,10 +44,12 @@ static short s16(float v) { return port_sat_s16i((int)lrintf(v)); }
 
 #define SRC(y, x, c) (depth == P_8U ? (float)((const uchar*)src + (size_t)(y) * sstep)[(x) * cn + (c)] : ((const float*)((const char*)src + (size_t)(y) * sstep))[(x) * cn + (c)])
 
-PORT_API int port_resize(const void* src, size_t sstep, int sw, int sh, void* dst, size_t dstep, int dw, int dh, int type, int interp)
+/* inv_x, inv_y: the inverse sampling scales hal::resize gets, dsize / ssize unless the caller gave fx, fy (resize.cpp:4214-4228) */
+static int resize_scaled(const void* src, size_t sstep, int sw, int sh, void* dst, size_t dstep, int dw, int dh, int type, int interp,
+                         double inv_x, double inv_y)
 {
     int depth = P_DEPTH(type), cn = P_CN(type), es = (int)port_esz(depth) * cn;
-    double inv_x = (double)dw / sw, inv_y = (double)dh / sh, scale_x = 1. / inv_x, scale_y = 1. / inv_y;
+    double scale_x = 1. / inv_x, scale_y = 1. / inv_y;
     if (depth != P_8U && depth != P_32F) return 1;
     if (dw == sw && dh == sh) {
         for (int y = 0; y < sh; y++) memcpy((char*)dst + (size_t)y * dstep, (const char*)src + (size_t)y * sstep, (size_t)sw * es);
@@ -77,9 +79,10 @@ PORT_API int port_resize(const void* src, size_t sstep, int sw, int sh, void* ds
                     } else {
                         const float* s0 = (const float*)((const char*)src + (size_t)(2 * y) * sstep) + 2 * x * cn + c;
                         const float* s1 = (const float*)((const char*)s0 + sstep);
-                        /* 4-lane SIMD body: (a+b)+(c+d); 3 channels and the single-channel remainder columns (dw % 4): scalar loop, ((a+b)+c)+d */
+                        /* 4-lane SIMD body: (a+b)+(c+d); 3 channels and the single-channel remainder columns (dw % 4): scalar loop,
+                         * sum = 0; sum += ((a+b)+c)+d -- -0 comes out as +0 */
                         int seq = cn == 3 || (cn == 1 && x >= (dw & ~3));
-                        float sum = seq ? ((s0[0] + s0[cn]) + s1[0]) + s1[cn] : (s0[0] + s0[cn]) + (s1[0] + s1[cn]);
+                        float sum = seq ? 0.f + (((s0[0] + s0[cn]) + s1[0]) + s1[cn]) : (s0[0] + s0[cn]) + (s1[0] + s1[cn]);
                         ((float*)((char*)dst + (size_t)y * dstep))[x * cn + c] = sum * 0.25f;
                     }
                 }
@@ -342,6 +345,21 @@ area_as_linear:;
             }
     free(xs); free(xa);
     return 0;
+}
+
+PORT_API int port_resize(const void* src, size_t sstep, int sw, int sh, void* dst, size_t dstep, int dw, int dh, int type, int interp)
+{
+    return resize_scaled(src, sstep, sw, sh, dst, dstep, dw, dh, type, interp, (double)dw / sw, (double)dh / sh);
+}
+
+/* cv::resize(src, dst, Size(), fx, fy): dst is round(sw * fx) x round(sh * fy), the sampling scales stay fx, fy.  NEAREST, LINEAR and
+ * CUBIC, and the exact 2 x 2 decimation on even sizes (the reference's partial last windows for odd sizes are not restated); 1 otherwise */
+PORT_API int port_resize_fxfy(const void* src, size_t sstep, int sw, int sh, void* dst, size_t dstep, int dw, int dh, int type, int interp,
+                              double fx, double fy)
+{
+    if (interp != 0 && interp != 1 && interp != 2) return 1;
+    if (fx == 0.5 && fy == 0.5 && interp == 1 && (2 * dw != sw || 2 * dh != sh)) return 1;
+    return resize_scaled(src, sstep, sw, sh, dst, dstep, dw, dh, type, interp, fx, fy);
 }
 
 /* ---- remap tables ---- */

@@ -6,9 +6,10 @@ Bars (the reference's own strict test allows |d| <= 1 for LINEAR/CUBIC, test_img
   warp* u8 (NEAREST/LINEAR/CUBIC) .......................... BIT-EXACT (fixed-point coordinates + 2^15 tap tables)
   f32 (resize and warps, every interpolation and border) ... BIT-EXACT: same float operations in the same order
 
-The warps here run at a few everyday geometries and at 8K.  tests/test_gpu_warp_exact.py takes each of the four warp kernels to its
-tile, column-block, footprint and alignment edges (table: tests/warp_cases.py; the port it compares with is held to the reference
-over the same table by tests/test_warp_port.py).
+Resize and the warps here run at a few everyday geometries and at 8K.  tests/test_gpu_warp_exact.py takes each of the four warp
+kernels to its tile, column-block, footprint and alignment edges (table: tests/warp_cases.py; the port it compares with is held to the
+reference over the same table by tests/test_warp_port.py); tests/test_gpu_resize_exact_edges.py does the same for every resize kernel
+(table: tests/resize_cases.py; port against reference: tests/test_resize_port.py).
 """
 import numpy as np
 import pytest
@@ -66,7 +67,7 @@ def test_resize_half_area(cvb, oracle, rng, interp):
         img = rand_u8(rng, 122, 250, cn)
         assert_exact(cpu(cvb.resize(gpu(img), (125, 61), interpolation=interp)), oracle.resize(img, (125, 61), interp), "half u8 cn=%d" % cn)
         f = img.astype(np.float32)
-        assert_close(cpu(cvb.resize(gpu(f), (125, 61), interpolation=interp)), oracle.resize(f, (125, 61), interp), atol=1e-4, what="half f32 cn=%d" % cn)
+        assert_exact(cpu(cvb.resize(gpu(f), (125, 61), interpolation=interp)), oracle.resize(f, (125, 61), interp), "half f32 cn=%d" % cn)
 
 
 @pytest.mark.parametrize("dsize,interp", [((3840, 2160), C.INTER_NEAREST), ((3840, 2160), C.INTER_LINEAR), ((5120, 2880), C.INTER_LINEAR),

@@ -732,3 +732,19 @@ def test_emulated_tiled_resize_vs_port(resize_sep_emu, port, rng):
     for cubic in (0, 1):
         got = resize_sep_emu(src, (113, 41), cubic, 16, pad=3)
         assert np.array_equal(got, port.resize(np.ascontiguousarray(src), (113, 41), 2 if cubic else 1)), "tiled resize, unaligned pitches, cubic=%d" % cubic
+
+
+def test_emulated_tiled_resize_edge_cases_vs_port(resize_sep_emu, port):
+    """the `sx` / `sy` / `am` cases of tests/resize_cases.py that run on resize_sep_u8_kernel, at the DH predict() names: no tile reads
+    more source rows than rs_host_rmax sized the shared memory for (the kernel clamps R to RMAX without a word; the emulation returns 77)"""
+    import resize_cases as rc
+    n = 0
+    for case in rc.CASES:
+        p = rc.predict(case)
+        if case.group not in ("sx", "sy", "am") or p.kernel != "resize_sep_u8_kernel":
+            continue
+        src = rc.frames_of(case)[0]
+        got = resize_sep_emu(src, case.dsize, case.interp == rc.CUBIC, p.DH, area_mode=int(case.interp == rc.AREA))
+        assert np.array_equal(got, port.resize(src, case.dsize, case.interp)), "%s at DH = %d" % (case.id, p.DH)
+        n += 1
+    assert n > 100
