@@ -193,7 +193,11 @@ B200CV_API int b200cv_pyr_up(const b200cvMat* src, const b200cvMat* dst, int bor
  * subsampled-YUV wire formats (codes 90-108, 111-112, 115-124, 127-134: NV12 / NV21 / YV12 / IYUV / UYVY / YUY2 / YVYU; color.cpp:323-380),
  * whose source and destination sizes differ: a 4:2:0 image of W x H pixels is one 8-bit plane of H*3/2 rows.
  * CV_16U and CV_32F images: the channel reorders (codes 0-5), BGR/RGB(A) <-> GRAY (6-11), BGR/RGB <-> XYZ (32-35), BGR/RGB <-> YCrCb / YUV (36-39, 82-85) and, float only, BGR/RGB <-> HSV (40-41, 54-55, 66-67, 70-71)
- * (color_rgb.simd.hpp:608-841, color_yuv.simd.hpp:134-396,616-1013, color_lab.cpp:172-700), bit-exact incl. float; other codes at those depths: NOT_IMPLEMENTED */
+ * (color_rgb.simd.hpp:608-841, color_yuv.simd.hpp:134-396,616-1013, color_lab.cpp:172-700), bit-exact incl. float; other codes at those depths: NOT_IMPLEMENTED.
+ * Bayer mosaics (1-channel source; demosaicing.cpp): bilinear to BGR / BGRA (46-49, 139-142) and edge-aware (135-138), 8- and 16-bit;
+ * Variable Number of Gradients (62-65), 8-bit to 3 channels only -- a 16-bit mosaic or a 4-channel destination is B200CV_ERR_BAD_ARG
+ * and leaves dst untouched; to GRAY (86-89), 8- and 16-bit.  Mosaics narrower or shorter than 3 pixels: NOT_IMPLEMENTED, except GRAY
+ * (all zero, as the reference).  Never in place. */
 B200CV_API int b200cv_cvt_color(const b200cvMat* src, const b200cvMat* dst, int code, void* stream);
 /* replaces cv::cvtColorTwoPlane (imgproc.hpp; color.cpp:171-185): NV12 / NV21 (codes 90-97) with the luma plane (8UC1, W x H) and the
  * interleaved chroma plane (8UC2, W/2 x H/2) in separate buffers with their own pitches, as hardware decoders hand them out */

@@ -50,6 +50,11 @@ COLOR_BayerBG2RGBA, COLOR_BayerGB2RGBA, COLOR_BayerRG2RGBA, COLOR_BayerGR2RGBA =
 # edge-aware demosaicing (demosaicing.cpp:1592-1737), 3-channel destinations
 COLOR_BayerBG2BGR_EA, COLOR_BayerGB2BGR_EA, COLOR_BayerRG2BGR_EA, COLOR_BayerGR2BGR_EA = 135, 136, 137, 138
 COLOR_BayerBG2RGB_EA, COLOR_BayerGB2RGB_EA, COLOR_BayerRG2RGB_EA, COLOR_BayerGR2RGB_EA = 137, 138, 135, 136
+# Variable Number of Gradients (demosaicing.cpp:1059-1587), 8-bit mosaics, 3-channel destinations
+COLOR_BayerBG2BGR_VNG, COLOR_BayerGB2BGR_VNG, COLOR_BayerRG2BGR_VNG, COLOR_BayerGR2BGR_VNG = 62, 63, 64, 65
+COLOR_BayerBG2RGB_VNG, COLOR_BayerGB2RGB_VNG, COLOR_BayerRG2RGB_VNG, COLOR_BayerGR2RGB_VNG = 64, 65, 62, 63
+# Bayer mosaic to luma (demosaicing.cpp:652-792), 8- and 16-bit
+COLOR_BayerBG2GRAY, COLOR_BayerGB2GRAY, COLOR_BayerRG2GRAY, COLOR_BayerGR2GRAY = 86, 87, 88, 89
 # subsampled-YUV wire formats (imgproc.hpp: ColorConversionCodes 90-134)
 COLOR_YUV2RGB_NV12, COLOR_YUV2BGR_NV12, COLOR_YUV2RGB_NV21, COLOR_YUV2BGR_NV21 = 90, 91, 92, 93
 COLOR_YUV2RGBA_NV12, COLOR_YUV2BGRA_NV12, COLOR_YUV2RGBA_NV21, COLOR_YUV2BGRA_NV21 = 94, 95, 96, 97
@@ -281,7 +286,7 @@ def Scharr(src, ddepth, dx, dy, scale=1.0, delta=0.0, borderType=BORDER_DEFAULT,
 
 _CVT_DCN = {COLOR_BGR2BGRA: 4, COLOR_BGRA2BGR: 3, COLOR_BGR2RGBA: 4, COLOR_RGBA2BGR: 3, COLOR_BGR2RGB: 3, COLOR_BGRA2RGBA: 4,
             COLOR_BGR2GRAY: 1, COLOR_RGB2GRAY: 1, COLOR_BGRA2GRAY: 1, COLOR_RGBA2GRAY: 1, COLOR_GRAY2BGR: 3, COLOR_GRAY2BGRA: 4,
-            139: 4, 140: 4, 141: 4, 142: 4}
+            139: 4, 140: 4, 141: 4, 142: 4, 86: 1, 87: 1, 88: 1, 89: 1}
 
 
 def _cvt_dst_geometry(code, cols, rows, dstCn=0):

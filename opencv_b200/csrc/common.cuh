@@ -149,6 +149,8 @@ int gauss_u16_sep_impl(const Img& s, const Img& d, int cn, const long long* fx, 
 int cvt_color_xyz(const b200cvMat* src, const b200cvMat* dst, int code, cudaStream_t st);        // cvtcolor_lab.cu
 int cvt_color_lab(const b200cvMat* src, const b200cvMat* dst, int code, cudaStream_t st);        // cvtcolor_lab.cu
 int demosaic_bilinear(const b200cvMat* src, const b200cvMat* dst, int code, cudaStream_t st);   // demosaic.cu
+int demosaic_gray(const b200cvMat* src, const b200cvMat* dst, int code, cudaStream_t st);       // demosaic.cu
+int demosaic_vng(const b200cvMat* src, const b200cvMat* dst, int code, cudaStream_t st);        // demosaic_vng.cu
 int cvt_color_two_plane(const b200cvMat* ysrc, const b200cvMat* uvsrc, const b200cvMat* dst, int code, cudaStream_t st);   // cvtcolor_yuv.cu
 int cvt_color_yuv(const b200cvMat* src, const b200cvMat* dst, int code, cudaStream_t st);      // cvtcolor_yuv.cu
 int cvt_color_depth(const b200cvMat* src, const b200cvMat* dst, int code, cudaStream_t st);    // cvtcolor_depth.cu (16U / 32F)

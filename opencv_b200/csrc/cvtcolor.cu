@@ -311,6 +311,10 @@ extern "C" int b200cv_cvt_color(const b200cvMat* src, const b200cvMat* dst, int 
         B200_REQUIRE(src->data != dst->data, "cvtColor: in-place is not supported");
         return demosaic_bilinear(src, dst, code, as_stream(stream));
     }
+    if ((code >= 62 && code <= 65) || (code >= 86 && code <= 89)) {       // Bayer VNG, 8-bit (demosaic_vng.cu); Bayer to GRAY, 8- and 16-bit (demosaic.cu)
+        B200_REQUIRE(src->data != dst->data, "cvtColor: in-place is not supported");
+        return code <= 65 ? demosaic_vng(src, dst, code, as_stream(stream)) : demosaic_gray(src, dst, code, as_stream(stream));
+    }
     if (B200CV_DEPTH(src->type) != B200CV_8U || B200CV_DEPTH(dst->type) != B200CV_8U) return cvt_color_depth(src, dst, code, as_stream(stream));   // 16U / 32F: cvtcolor_depth.cu
     const int scn = B200CV_CN(src->type), dcn = B200CV_CN(dst->type);
     Img s = make_img(src), d = make_img(dst);

@@ -1,6 +1,6 @@
 // demosaic.cu -- cv::cvtColor / cv::demosaicing for the Bayer patterns, bilinear and edge-aware interpolation, 8- and 16-bit (the
 // wire format of a raw sensor).  Codes COLOR_BayerBG/GB/RG/GR2BGR = 46..49 (the 2RGB names are the same numbers permuted), 2BGRA = 139..142,
-// 2BGR_EA = 135..138.
+// 2BGR_EA = 135..138, and Bayer to GRAY, 2GRAY = 86..89 (VNG, 62..65, is demosaic_vng.cu).
 //
 // Reference (demosaicing.cpp:806-1056, Bayer2RGB_Invoker / Bayer2RGB_): for every interior pixel of the mosaic
 //   at a red / blue site:  that colour = the sample, green = (4 edge neighbours + 2) >> 2, the other colour = (4 diagonal neighbours + 2) >> 2
@@ -68,7 +68,69 @@ __global__ void __launch_bounds__(256) bayer_bilinear_kernel(Img src, Img dst, i
     }
 }
 
+// Bayer2Gray_ (demosaicing.cpp:652-792): at a red / blue site (4 diagonal neighbours * rcoeff + 4 edge neighbours * G2Y + 4 * sample * bcoeff
+// + 2^15) >> 16, at a green site (2 vertical neighbours * rcoeff + 2 horizontal neighbours * bcoeff + 2 * G2Y * sample + 2^14) >> 15; rcoeff
+// and bcoeff swap and start_with_green flips every interior row.  Unsigned sums: a 16-bit mosaic reaches 4 294 934 528 > INT_MAX.  The
+// reference's 8-bit vector body (:180-272) is the same arithmetic scaled by 2.  Border pixels repeat the nearest interior site; an image
+// with W <= 2 or H <= 2 is all zero (:695-699, :789-791).  Eight destination pixels per thread.
+template <typename T>
+__global__ void __launch_bounds__(256) bayer_gray_kernel(Img src, Img dst, int W, int H, unsigned b0, unsigned r0, int swg0)
+{
+    const int x0 = (blockIdx.x * blockDim.x + threadIdx.x) * 8;
+    const int y = blockIdx.y, f = blockIdx.z;
+    if (x0 >= W) return;
+    const int n = min(8, W - x0);
+    union { T e[8]; uchar b[8 * sizeof(T)]; } o;
+    if (W <= 2 || H <= 2) {
+#pragma unroll
+        for (int j = 0; j < 8; j++) o.e[j] = 0;
+    } else {
+        const unsigned G2Y = 9617;
+        const int yi = min(max(y, 1), H - 2), i = yi - 1;
+        const unsigned bco = (i & 1) ? r0 : b0, rco = (i & 1) ? b0 : r0;
+        const bool swg = ((i & 1) != 0) != (swg0 != 0);
+        const T* q0 = src.row<T>(f, yi - 1);
+        const T* q1 = src.row<T>(f, yi);
+        const T* q2 = src.row<T>(f, yi + 1);
+#pragma unroll
+        for (int j = 0; j < 8; j++) {
+            const int xi = min(max(min(x0 + j, W - 1), 1), W - 2), k = xi - 1;
+            const T *r0p = q0 + xi, *r1 = q1 + xi, *r2 = q2 + xi;
+            unsigned v;
+            if (((k & 1) == 0) == swg)
+                v = ((unsigned)(r0p[0] + r2[0]) * rco + (unsigned)(r1[-1] + r1[1]) * bco + (unsigned)r1[0] * (2 * G2Y) + (1u << 14)) >> 15;
+            else
+                v = ((unsigned)(r0p[-1] + r0p[1] + r2[-1] + r2[1]) * rco + (unsigned)(r0p[0] + r1[-1] + r1[1] + r2[0]) * G2Y + (unsigned)r1[0] * (4 * bco)
+                     + (1u << 15)) >> 16;
+            o.e[j] = (T)v;
+        }
+    }
+    uchar* dp = dst.row<uchar>(f, y) + (size_t)x0 * sizeof(T);
+    if constexpr (sizeof(T) == 1) store_bytes<8>(dp, n, o.b);
+    else store_bytes<16>(dp, n * 2, o.b);
+}
+
 }  // namespace
+
+// called by b200cv_cvt_color for codes 86-89 (matrices of equal size and batch, not in place, already checked); 8- and 16-bit
+int demosaic_gray(const b200cvMat* src, const b200cvMat* dst, int code, cudaStream_t st)
+{
+    const int depth = B200CV_DEPTH(src->type);
+    if ((depth != B200CV_8U && depth != B200CV_16U) || B200CV_DEPTH(dst->type) != depth) return B200CV_NOT_IMPLEMENTED;
+    B200_REQUIRE(B200CV_CN(src->type) == 1 && B200CV_CN(dst->type) == 1, "Bayer -> GRAY needs a 1-channel mosaic and a 1-channel destination");
+    Img s = make_img(src), d = make_img(dst);
+    const int W = src->cols, H = src->rows;
+    if (H >= 65536 || s.frames >= 65536) return B200CV_NOT_IMPLEMENTED;
+    const unsigned R2Y = 4899, B2Y = 1868;
+    const int c = code - 86;                                            // 0 BG, 1 GB, 2 RG, 3 GR
+    const unsigned b0 = c < 2 ? B2Y : R2Y, r0 = c < 2 ? R2Y : B2Y;
+    const dim3 block(256);
+    const dim3 grid(div_up(div_up((unsigned)W, 8), 256), (unsigned)H, (unsigned)s.frames);
+    if (depth == B200CV_8U) bayer_gray_kernel<uchar><<<grid, block, 0, st>>>(s, d, W, H, b0, r0, c & 1);
+    else bayer_gray_kernel<unsigned short><<<grid, block, 0, st>>>(s, d, W, H, b0, r0, c & 1);
+    B200_LAUNCH_CHECK();
+    return B200CV_OK;
+}
 
 // called by b200cv_cvt_color for codes 46-49, 135-138 (edge-aware) and 139-142 (matrices of equal size and batch already checked); 8- and 16-bit
 int demosaic_bilinear(const b200cvMat* src, const b200cvMat* dst, int code, cudaStream_t st)

@@ -183,6 +183,7 @@ inline void cvtColorGeometry(int code, int cols, int rows, int dcn, int& w, int&
     else if (code >= 127 && code <= 134) { h = rows * 3 / 2; cn = 1; }
     else if (code >= 143 && code <= 154) cn = 2;
     else if (code >= 139 && code <= 142) cn = 4;
+    else if (code >= 86 && code <= 89) cn = 1;
     else if (cn <= 0) cn = (code == 0 || code == 2 || code == 5 || code == 9) ? 4 : (code == 6 || code == 7 || code == 10 || code == 11) ? 1 : 3;
 }
 inline void cvtColor(const GpuMat& src, GpuMat& dst, int code, int dcn = 0, Stream& s = Stream::Null())
