@@ -155,7 +155,6 @@ int cvt_color_two_plane(const b200cvMat* ysrc, const b200cvMat* uvsrc, const b20
 int cvt_color_yuv(const b200cvMat* src, const b200cvMat* dst, int code, cudaStream_t st);      // cvtcolor_yuv.cu
 int cvt_color_depth(const b200cvMat* src, const b200cvMat* dst, int code, cudaStream_t st);    // cvtcolor_depth.cu (16U / 32F)
 int gauss_u8_binomial(const Img& s, const Img& d, int cn, const int64_t* fx, int kw, const int64_t* fy, int kh, int border, cudaStream_t st);   // gauss_u8_binomial.cu
-int gauss_u8_march(const Img& s, const Img& d, int KB, const unsigned char* tx, const unsigned char* ty, int border, cudaStream_t st, int sep_mode, int even_limit);   // gauss_u8_march.cu
 int gauss_u8_fast(const Img& s, const Img& d, int cn, const int64_t* fx, int kw, const int64_t* fy, int kh, int border, cudaStream_t st, int sep_mode = 0, int even_limit = 0,
                   const GU8Box* box = nullptr);
 

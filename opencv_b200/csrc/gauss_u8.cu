@@ -282,14 +282,10 @@ int gauss_u8_fast(const Img& s, const Img& d, int cn, const int64_t* fx, int kw,
     for (int i = 0; i < kh; i++) sy += fy[i];
     if (sx > 256 || sy > 256) return B200CV_NOT_IMPLEMENTED;      // 16-bit row sums and an unsaturated result byte
     // GaussianBlur 3 x 3 / 5 x 5 with the binomial 8.8 taps (sigma = 0), one channel, 16-byte aligned rows of a multiple of 16 pixels: packed
-    // 16-bit adds, no multiplier, rows through a lane-private cp.async ring (gauss_u8_binomial.cu).  The TMA tile kernel below keeps every other case
-    // and is forced by B200CV_GAUSS_U8_PATH=tile (tests run both)
+    // 16-bit adds, no multiplier, rows through a lane-private cp.async ring (gauss_u8_binomial.cu).  Every other case runs on the TMA tile kernel below
     if (sep_mode == 0 && !box) {
-        const char* e = getenv("B200CV_GAUSS_U8_PATH");
-        if (!(e && (!strcmp(e, "tile") || !strcmp(e, "stream")))) {
-            const int brc = gauss_u8_binomial(s, d, cn, fx, kw, fy, kh, border, st);
-            if (brc != B200CV_NOT_IMPLEMENTED) return brc;
-        }
+        const int brc = gauss_u8_binomial(s, d, cn, fx, kw, fy, kh, border, st);
+        if (brc != B200CV_NOT_IMPLEMENTED) return brc;
     }
     GU8Params p;
     memset(&p, 0, sizeof(p));
@@ -303,13 +299,6 @@ int gauss_u8_fast(const Img& s, const Img& d, int cn, const int64_t* fx, int kw,
             for (int i = 0; i < 4; i++) { int j = 4 * g + i - o; if (j >= 0 && j < KB) w |= (uint32_t)ty[j] << (8 * i); }
             p.kyw[o][g] = w;
         }
-    // single channel, K <= 9, Gaussian / 8.8 sepFilter2D epilogues: the warp-streaming register kernel (gauss_u8_march.cu) exists as a second
-    // version; it executes fewer instructions per pixel but gives the memory system less in flight (per-warp chunks), so the tile kernel
-    // below stays the default; B200CV_GAUSS_U8_PATH=stream selects it (tests run both)
-    {
-        const char* e = getenv("B200CV_GAUSS_U8_PATH");
-        if (e && !strcmp(e, "stream") && cn == 1 && KB <= 9 && sep_mode <= 1) return gauss_u8_march(s, d, KB, tx, ty, border, st, sep_mode, even_limit);
-    }
     p.W = s.cols * cn; p.H = s.rows; p.border = border; p.sep_mode = sep_mode; p.even_limit = even_limit;      // W in byte elements
     if (box) p.box = *box;
     p.TH = ((64 - (KB - 1)) / 4) * 4;

@@ -1,6 +1,5 @@
 // hal_api.cu -- host-pointer entry points: the cv_hal_* replacement functions and the batched host pipeline.
 // No arithmetic here: upload, call the device API of b200cv.h, download.
-#include <cstdlib>
 #include <functional>
 #include <vector>
 #include "common.cuh"
@@ -8,7 +7,8 @@
 
 namespace b200cv {
 
-constexpr int NPIPE = 4;          // pipeline streams (B200CV_HOST_PIPE=1..4 overrides; default 3)
+constexpr int NPIPE = 3;                            // host pipeline streams
+constexpr size_t CHUNK_BYTES = (size_t)32 << 20;    // upload + download bytes per chunk of frames (at least one frame per chunk)
 
 struct HostCtx {                      // one per host thread: OpenCV calls HAL functions concurrently from many threads
     cudaStream_t st[NPIPE] = {};
@@ -53,13 +53,11 @@ static int host_pipeline(const b200cvMat* hsrc, const b200cvMat* hdst, const Dev
     const size_t sp = pitch_of(hsrc), dp = pitch_of(hdst);
     const size_t sfb = sp * hsrc->rows, dfb = dp * hdst->rows;
     // chunk so that a chunk is ~>= 32 MB of traffic but at least 1 frame; single frames use one stream
-    static const int env_pipe = [] { const char* e = getenv("B200CV_HOST_PIPE"); int v = e ? atoi(e) : 3; return v < 1 ? 1 : v > NPIPE ? NPIPE : v; }();
-    static const size_t env_chunk = [] { const char* e = getenv("B200CV_HOST_CHUNK_MB"); int v = e ? atoi(e) : 32; return (size_t)(v < 1 ? 1 : v) << 20; }();
-    int chunk = (int)std::max<size_t>(1, env_chunk / std::max<size_t>(1, sfb + dfb));
+    int chunk = (int)std::max<size_t>(1, CHUNK_BYTES / std::max<size_t>(1, sfb + dfb));
     if (chunk > frames) chunk = frames;
     HostCtx& c = g_ctx;
     const int nchunks = (frames + chunk - 1) / chunk;
-    const int npipe = nchunks < env_pipe ? nchunks : env_pipe;
+    const int npipe = nchunks < NPIPE ? nchunks : NPIPE;
     for (int i = 0; i < npipe; i++) {
         if (!c.st[i]) B200_CUDA(cudaStreamCreateWithFlags(&c.st[i], cudaStreamNonBlocking));
         if ((rc = ensure(&c.dbuf[i][0], &c.cap[i][0], sfb * chunk)) || (rc = ensure(&c.dbuf[i][1], &c.cap[i][1], dfb * chunk))) return rc;

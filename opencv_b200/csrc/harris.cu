@@ -15,7 +15,6 @@
 // per frame; a frame with more (a noise frame at 8K has ~2 10^6, a plateau frame up to (W - 2)(H - 2)) makes the list grow to the
 // largest count and the candidates be found a second time, so no candidate is ever dropped.
 #include <algorithm>
-#include <chrono>
 #include <cstdio>
 #include <cmath>
 #include <cstdlib>
@@ -630,9 +629,6 @@ extern "C" int b200cv_good_features_to_track(const b200cvMat* src, float* corner
     int rc;
     if ((rc = check_mat(src, "src"))) return rc;
     B200_REQUIRE(corners && counts && max_out > 0, "bad output arguments");
-    const bool trace = getenv("B200CV_GFTT_TRACE") != nullptr;
-    auto t_last = std::chrono::steady_clock::now();
-    auto lap = [&](const char* what) { if (!trace) return; auto t = std::chrono::steady_clock::now(); fprintf(stderr, "gftt %-14s %8.1f us\n", what, std::chrono::duration<double, std::micro>(t - t_last).count()); t_last = t; };
     B200_REQUIRE(quality_level > 0 && min_distance >= 0 && max_corners >= 0, "bad parameters");
     const int W = src->cols, H = src->rows, frames = src->frames > 1 ? src->frames : 1;
     cudaStream_t st = as_stream(stream);
@@ -690,10 +686,7 @@ extern "C" int b200cv_good_features_to_track(const b200cvMat* src, float* corner
         }
         if ((ce = cudaMemcpyAsync(hcnt.data(), d_cnt, sizeof(int) * frames, cudaMemcpyDeviceToHost, st)) != cudaSuccess) return ce;
         if (preselect && (ce = cudaMemcpyAsync(hsel.data(), d_topcnt, sizeof(int) * frames, cudaMemcpyDeviceToHost, st)) != cudaSuccess) return ce;
-        lap("enqueue 1");
-        ce = cudaStreamSynchronize(st);
-        lap("sync 1");
-        return ce;
+        return cudaStreamSynchronize(st);
     };
     TRY(find_candidates());
     // a frame with more candidates than the list holds (noise or plateaus at 8K: up to (W - 2)(H - 2)): every candidate is kept -- the
@@ -736,8 +729,7 @@ extern "C" int b200cv_good_features_to_track(const b200cvMat* src, float* corner
     static thread_local Side side;
     int cur_dev = 0;
     TRY(cudaGetDevice(&cur_dev));
-    const char* ss_env = getenv("B200CV_GFTT_STREAMS");                          // "1": the sorts queue on the caller's stream one after the other
-    const int ns = (ss_env && ss_env[0] == '1') ? 1 : std::min(frames, NSIDE);
+    const int ns = std::min(frames, NSIDE);
     if (ns > 1 && side.dev != cur_dev) {
         if (side.dev >= 0) { for (int i = 0; i < NSIDE; i++) { cudaStreamDestroy(side.s[i]); cudaEventDestroy(side.join[i]); } cudaEventDestroy(side.fork); side.dev = -1; }
         for (int i = 0; i < NSIDE; i++) { TRY(cudaStreamCreateWithFlags(&side.s[i], cudaStreamNonBlocking)); TRY(cudaEventCreateWithFlags(&side.join[i], cudaEventDisableTiming)); }
@@ -765,9 +757,7 @@ extern "C" int b200cv_good_features_to_track(const b200cvMat* src, float* corner
         if (ns > 1)
             for (int i = 0; i < ns; i++) { TRY(cudaEventRecord(side.join[i], side.s[i])); TRY(cudaStreamWaitEvent(st, side.join[i], 0)); }
     }
-    lap("enqueue 2");
     TRY(cudaStreamSynchronize(st));
-    lap("sync 2");
     std::vector<CandKey> chunk;
     std::vector<int> head, nxt;                  // accepted corners per grid cell: singly linked lists in flat arrays
     std::vector<float> ax, ay;
@@ -840,8 +830,6 @@ extern "C" int b200cv_good_features_to_track(const b200cvMat* src, float* corner
       }
     }
 #undef TRY
-    lap("walk");
     cleanup2();
-    lap("free");
     return B200CV_OK;
 }

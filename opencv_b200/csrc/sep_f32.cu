@@ -481,7 +481,6 @@ static int launch_sf32(const CUtensorMap& tm, const CUtensorMap& tm_tail, const 
     // chunks per CTA: 4 (128 rows) for 13 taps and more when the grid stays several waves deep; small kernels keep the plain tile form
     const long tiles = (long)div_up((unsigned)p.W, SF_TW) * div_up((unsigned)p.H, SF_TH) * frames;
     p.nch = (KB >= 13 && tiles >= 8L * 2 * num_sms()) ? 4 : (KB >= 13 && tiles >= 4L * 2 * num_sms()) ? 2 : 1;
-    if (p.has_dog && getenv("B200CV_SEP_DOG_TILE")) p.nch = 1;      // measurement switch: the plain tile kernel for the fused-DoG blurs
     auto kern = sep_f32_tma_kernel<KB, ST, DT, SKIP0>;
     static PerDeviceFlag attr_pd; bool& attr = attr_pd.cur();
     if (!attr) { B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = true; }

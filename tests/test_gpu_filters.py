@@ -347,28 +347,12 @@ def test_filter2d_generic(cvb, oracle, rng):
     assert_exact(cpu(cvb.filter2D(gpu(img3), 5, ker)), oracle.filter2D(img3, 5, ker), "filter2D u8->f32 (24 taps: direct sum, scalar order)")
 
 
-@pytest.mark.parametrize("k", [3, 5, 7, 9])
-def test_gaussian_u8_streaming_kernel(cvb, oracle, rng, monkeypatch, k):
-    """the warp-streaming second version of the 8-bit Gaussian (gauss_u8_march.cu; B200CV_GAUSS_U8_PATH=stream -- the tile kernel
-    stays the default): bit-exact like the default path, every border, ragged sizes, a batch, and sepFilter2D's 8.8 mode"""
-    monkeypatch.setenv("B200CV_GAUSS_U8_PATH", "stream")
-    for shape in ((3, 211, 333, 1), (1, 64, 224, 1), (2, 37, 1000, 1)):
-        img = rng.integers(0, 256, shape, dtype=np.uint8)
-        for border in (4, 1, 0, 2):      # REFLECT_101, REPLICATE, CONSTANT, REFLECT
-            got = cpu(cvb.GaussianBlur(gpu(img), (k, k), 0, borderType=border))
-            for f in range(shape[0]):
-                assert_exact(got[f, :, :, 0], oracle.GaussianBlur(img[f, :, :, 0], (k, k), 0, borderType=border), "stream Gaussian k=%d border=%d" % (k, border))
-    t = cvb.getGaussianKernel(k, 0).astype(np.float32)
-    img = rng.integers(0, 256, (180, 300), dtype=np.uint8)
-    assert_exact(cpu(cvb.sepFilter2D(gpu(img), -1, t, t)), oracle.sepFilter2D(img, -1, t, t), "stream sepFilter2D 8.8 mode k=%d" % k)
-
-
 @pytest.mark.parametrize("k", [3, 5])
 @pytest.mark.parametrize("width", [32, 48, 131, 512, 528, 1022, 2064])
-def test_gaussian_u8_binomial_kernel(cvb, oracle, rng, monkeypatch, k, width):
-    """3 x 3 / 5 x 5 sigma = 0 on one channel: the packed 16-bit binomial kernel (gauss_u8_binomial.cu; the default where it applies, B200CV_GAUSS_U8_PATH=tile forces the general kernel) on views of a wider
-    buffer (16-byte aligned rows; widths that are multiples of 16 run it, the others fall through to the tile kernel); every border mode it takes;
-    part-filled last warps (48, 528, 2064); equal to the oracle and to the tile kernel"""
+def test_gaussian_u8_binomial_kernel(cvb, oracle, rng, k, width):
+    """3 x 3 / 5 x 5 sigma = 0 on one channel, on views of a wider buffer (16-byte aligned rows): widths that are multiples of 16 run the
+    packed 16-bit binomial kernel (gauss_u8_binomial.cu), the others (131, 1022) the TMA tile kernel; every border mode the binomial kernel
+    takes; part-filled last warps (48, 528, 2064); equal to the oracle"""
     import torch
     h = 70
     base = gpu(rand_u8(rng, h, ((width + 15) // 16) * 16 + 16))
@@ -377,8 +361,5 @@ def test_gaussian_u8_binomial_kernel(cvb, oracle, rng, monkeypatch, k, width):
     outb = torch.zeros_like(base)
     for b in (0, 1, 2, 4):
         want = oracle.GaussianBlur(img, (k, k), 0, 0, b)
-        monkeypatch.delenv("B200CV_GAUSS_U8_PATH", raising=False)
         got = cpu(cvb.GaussianBlur(view, (k, k), 0, 0, b, dst=outb[:, :width]))
         assert_exact(got, want, "binomial k=%d w=%d border=%d" % (k, width, b))
-        monkeypatch.setenv("B200CV_GAUSS_U8_PATH", "tile")
-        assert_exact(cpu(cvb.GaussianBlur(view, (k, k), 0, 0, b)), want, "tile kernel k=%d w=%d border=%d" % (k, width, b))

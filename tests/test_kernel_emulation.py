@@ -596,75 +596,6 @@ def test_emulated_gaussian_u16_vs_port(gauss16_emu, port, rng):
         assert list(C.getGaussianKernelFixed(k, s, 16)) == list(want) and int(want.sum()) == 65536, "16-bit taps k=%d sigma=%g" % (k, s)
 
 
-# ---- GaussianBlur / 8.8 sepFilter2D CV_8UC1, K <= 9: the warp-streaming kernel (gauss_u8_march.cu) ------------------------------------------
-# TMA and mbarriers cannot run on the host; everything a lane does with a staged chunk can.  The test walks the kernel's own work
-# decomposition (items -> chunks), stages every 256 x CH chunk with cv::borderInterpolate (what the TMA zero fill, the row-wise mirrored
-# loads and the apron patch produce together) and runs gm_lane_chunk for the 32 lanes, each with its register window carried across chunks.
-@pytest.fixture(scope="module")
-def gauss_march_emu(port):
-    body = r"""
-    using namespace b200cv;
-    Img si = make_img(s), di = make_img(d);
-    GMParams p; gm_fill_params(p, KB, tx, ty);
-    p.W = si.cols; p.H = si.rows; p.border = border; p.sep_mode = sep_mode; p.even_limit = even_limit;
-    const int H = KB / 2, CH = KB == 3 ? GMCfg<3>::CH : KB == 5 ? GMCfg<5>::CH : KB == 7 ? GMCfg<7>::CH : GMCfg<9>::CH;
-    p.tiles_x = (p.W + GM_OW - 1) / GM_OW;
-    p.seg_rows = ((seg_rows + CH - 1) / CH) * CH; p.nseg = (p.H + p.seg_rows - 1) / p.seg_rows; p.nitems = p.tiles_x * p.nseg * si.frames;
-    unsigned char* buf = (unsigned char*)malloc((size_t)GM_IW * CH);
-#define RUN(K, SEP) do { for (int item = 0; item < p.nitems; item++) { const GMItem g = gm_item<K>(p, item); \
-        for (int lane = 0; lane < 32; lane++) { uint32_t win[GMCfg<K>::NP][8]; memset(win, 0x5A, sizeof(win)); \
-            for (int chunk = 0; chunk < g.nchunks; chunk++) { \
-                for (int r = 0; r < CH; r++) for (int c = 0; c < GM_IW; c++) { \
-                    const int gy = g.ys - H + chunk * CH + r, gx = g.x0 - GM_RA + c; \
-                    const int sy = border_interpolate(gy, p.H, border), sx = border_interpolate(gx, p.W, border); \
-                    buf[r * GM_IW + c] = (sy < 0 || sx < 0) ? 0 : si.row<unsigned char>(g.f, sy)[sx]; } \
-                gm_lane_chunk<K, SEP>(buf, lane, p, di, g, chunk, win); } } } } while (0)
-    if (sep_mode) { if (KB == 3) RUN(3, true); else if (KB == 5) RUN(5, true); else if (KB == 7) RUN(7, true); else RUN(9, true); }
-    else { if (KB == 3) RUN(3, false); else if (KB == 5) RUN(5, false); else if (KB == 7) RUN(7, false); else RUN(9, false); }
-    free(buf);
-    return 0;"""
-    lib = build_emulation_raw("gauss_u8_march.cu", "int emu_gauss_march(const b200cvMat* s, const b200cvMat* d, int KB, const unsigned char* tx, const unsigned char* ty, int border, int sep_mode, int even_limit, int seg_rows)", body)
-
-    def run(img, k, sigma, border, sep=False, seg_rows=64):
-        fx = np.zeros(k, np.int64)
-        port.lib.port_gaussian_taps_fixed(k, ctypes.c_double(sigma), 8, fx.ctypes.data_as(ctypes.c_void_p))
-        assert fx.sum() == 256 and fx.max() <= 255
-        t = fx.astype(np.uint8)
-        dst = np.full_like(img, 0xCD)
-        ms, md = mat_of(img), mat_of(dst)
-        even_limit = (img.shape[-1] // 16) * 16 if sep else 0           # sepfilter.cu: ((cols * cn) / 16) * 16
-        rc = lib.emu_gauss_march(ctypes.byref(ms), ctypes.byref(md), k, t.ctypes.data_as(ctypes.c_void_p), t.ctypes.data_as(ctypes.c_void_p), border, int(sep), even_limit, seg_rows)
-        assert rc == 0
-        return (dst, (t / 256.0).astype(np.float32)) if sep else dst
-    return run
-
-
-def test_emulated_gaussian_march_vs_port(gauss_march_emu, port, rng):
-    for shape in [(37, 53), (150, 250), (131, 224), (300, 449), (200, 448), (2, 40, 230, 1)]:
-        img = rng.integers(0, 256, shape, dtype=np.uint8)
-        ext = np.where(rng.random(shape) < 0.5, 0, 255).astype(np.uint8)
-        for im in (img, ext):
-            for k, s in [(3, 0), (5, 0), (7, 0), (9, 0), (5, 1.7), (9, 2.5)]:
-                for border in (4, 1, 0, 2):
-                    got = gauss_march_emu(im, k, s, border, seg_rows=(64 if border != 1 else 1000))
-                    if im.ndim == 4:
-                        want = np.stack([port.GaussianBlur(im[i, :, :, 0], (k, k), s, s, border) for i in range(im.shape[0])])[..., None]
-                    else:
-                        want = port.GaussianBlur(im, (k, k), s, s, border)
-                    assert np.array_equal(got, want), "u8 march %s k=%d s=%g border=%d" % (shape, k, s, border)
-
-
-def test_emulated_sepfilter_8p8_march_vs_port(gauss_march_emu, port, rng):
-    """sepFilter2D's 8.8 fixed-point mode on the same kernel: half-to-even in the reference's vector body, half-up in its tail"""
-    for shape in [(37, 53), (150, 250), (64, 241)]:
-        img = rng.integers(0, 256, shape, dtype=np.uint8)
-        for k, s in [(3, 0), (5, 0), (7, 0), (9, 0)]:
-            for border in (4, 1, 0, 2):
-                got, taps = gauss_march_emu(img, k, s, border, sep=True)
-                want = port.sepFilter2D(img, -1, taps, taps, borderType=border)
-                assert np.array_equal(got, want), "u8 8.8 sepFilter2D march %s k=%d border=%d" % (shape, k, border)
-
-
 # ---- cv::resize INTER_LINEAR / INTER_CUBIC, 8-bit, tiled separable kernels (resize_sep.cu) ----------------------------------------------------
 # The kernel's shared-memory tile becomes a plain array; the H pass runs for all 256 threads, then the V pass (what the barrier separates).
 @pytest.fixture(scope="module")
