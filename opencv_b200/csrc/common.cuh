@@ -145,7 +145,6 @@ int resize_exact_impl(const Img& s, const Img& d, int depth, int cn, int interpo
 int resize_area_impl(const Img& s, const Img& d, int depth, int cn, cudaStream_t st);           // resize_area.cu
 int integral_impl(const b200cvMat* src, const b200cvMat* sum, const b200cvMat* sqsum, cudaStream_t st);   // integral.cu
 int gauss_u16_impl(const Img& s, const Img& d, int cn, const long long* fx, int kw, const long long* fy, int kh, int border, cudaStream_t st);   // gauss_u16.cu
-int gauss_u16_sep_impl(const Img& s, const Img& d, int cn, const long long* fx, int kw, const long long* fy, int kh, int border, cudaStream_t st);   // gauss_u16_sep.cu
 int cvt_color_xyz(const b200cvMat* src, const b200cvMat* dst, int code, cudaStream_t st);        // cvtcolor_lab.cu
 int cvt_color_lab(const b200cvMat* src, const b200cvMat* dst, int code, cudaStream_t st);        // cvtcolor_lab.cu
 int demosaic_bilinear(const b200cvMat* src, const b200cvMat* dst, int code, cudaStream_t st);   // demosaic.cu

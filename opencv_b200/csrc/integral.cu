@@ -1,24 +1,19 @@
-// integral.cu -- cv::integral for 8UC1 images: sum (CV_32S) and, optionally, the sum of squares (CV_64F) .
+// integral.cu -- cv::integral for 8UC1 images: sum (CV_32S) and, optionally, the sum of squares (CV_64F).
 //
 // Reference (sumpixels.dispatch.cpp:192-235, :415-451): sum is (H+1) x (W+1), first row and column zero,
 //     sum[y+1][x+1] = sum[y][x+1] + (src[y][0] + ... + src[y][x]);  int arithmetic (it wraps for images beyond 2^31 / 255 pixels, as the
 //     reference's does); squares accumulate in double, where every partial sum is an integer below 2^53: exact in any order.
-// Six small kernels, none of which needs threads to talk to each other (every stage is a map over independent pieces, so the whole op
-// also runs under the host emulation of tests/):
-//   rows:     H1 sum of every 16-pixel chunk            H2 exclusive scan of the chunk sums of a row      H3 prefix inside the chunk + offset -> sum
-//   columns:  V1 sum of every 32-row block of a column  V2 exclusive scan of the block sums of a column   V3 prefix inside the block + offset, in place
-// Algorithmic traffic: 1 byte read + 4 (12 with squares) written per pixel; this version re-reads the source once and the output twice.
-#include <stdlib.h>
-#include <string.h>
+// Two kernels with warp scans:
+//   rows     one warp per (frame, row): 128 pixels per step -- a 32-bit load of 4 pixels per lane, the prefix of the 4 in the lane, an
+//            inclusive shuffle scan of the lane totals, the running total of the row carried from step to step -- written as row prefixes to
+//            sum[y + 1][1 ..]; the same kernel zeroes column 0 and row 0
+//   columns  one thread per column walks down the image adding in place, 8 rows of loads in flight; coalesced across the threads of a warp
+// Traffic: 1 byte read + 4 written (rows) + 4 read + 4 written (columns) = 13 bytes per pixel against 5 algorithmic.
 #include "common.cuh"
 
 namespace b200cv {
 
-int integral_scan_run(const Img& s, const Img& o, int squares, cudaStream_t st);      // integral_scan.cu
-
 namespace {
-
-enum { IG_CHUNK = 16, IG_ROWS = 32 };
 
 template <typename T, bool SQ> __device__ __forceinline__ T ig_val(uchar v)
 {
@@ -26,124 +21,85 @@ template <typename T, bool SQ> __device__ __forceinline__ T ig_val(uchar v)
     else return (T)v;
 }
 
-struct IgDims { int W, H, NC, NB; };
+template <typename T> __device__ __forceinline__ T ig_shfl_up(T v, int d)
+{
+    if constexpr (sizeof(T) == 8) {
+        const long long b = __double_as_longlong((double)v);
+        const int lo = __shfl_up_sync(0xffffffffu, (int)(b & 0xffffffffll), d), hi = __shfl_up_sync(0xffffffffu, (int)(b >> 32), d);
+        return (T)__longlong_as_double(((long long)hi << 32) | (unsigned)lo);
+    } else return (T)__shfl_up_sync(0xffffffffu, (int)v, d);
+}
+template <typename T> __device__ __forceinline__ T ig_shfl(T v, int l)
+{
+    if constexpr (sizeof(T) == 8) {
+        const long long b = __double_as_longlong((double)v);
+        const int lo = __shfl_sync(0xffffffffu, (int)(b & 0xffffffffll), l), hi = __shfl_sync(0xffffffffu, (int)(b >> 32), l);
+        return (T)__longlong_as_double(((long long)hi << 32) | (unsigned)lo);
+    } else return (T)__shfl_sync(0xffffffffu, (int)v, l);
+}
 
 template <typename T, bool SQ>
-__global__ void __launch_bounds__(256) integral_h1_kernel(Img src, T* cs, IgDims g)
+__global__ void __launch_bounds__(256) integral_rows_kernel(Img src, Img out, int W, int H)
 {
-    const int c = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y, f = blockIdx.z;
-    if (c >= g.NC) return;
-    const uchar* s = src.row<uchar>(f, y) + c * IG_CHUNK;
-    const int n = min((int)IG_CHUNK, g.W - c * IG_CHUNK);
-    T acc = 0;
-    for (int i = 0; i < n; i++) acc += ig_val<T, SQ>(s[i]);
-    cs[((size_t)f * g.H + y) * g.NC + c] = acc;
+    const int lane = threadIdx.x & 31;
+    const int y = blockIdx.x * 8 + (threadIdx.x >> 5), f = blockIdx.y;
+    if (y >= H) return;
+    const uchar* s = src.row<uchar>(f, y);
+    T* o = out.row<T>(f, y + 1) + 1;
+    const bool al = (((uintptr_t)s) & 3) == 0;
+    if (lane == 0) o[-1] = 0;                                       // first column
+    if (y == 0) { T* z = out.row<T>(f, 0); for (int x = lane; x <= W; x += 32) z[x] = 0; }      // first row
+    T carry = 0;
+    for (int x0 = 0; x0 < W; x0 += 128) {
+        const int x = x0 + 4 * lane;
+        unsigned w = 0;
+        if (x + 4 <= W && al) w = __ldg((const unsigned*)(s + x));
+        else {
+#pragma unroll
+            for (int i = 0; i < 4; i++) if (x + i < W) w |= (unsigned)s[x + i] << (8 * i);
+        }
+        T p0 = ig_val<T, SQ>((uchar)(w & 255)), p1 = p0 + ig_val<T, SQ>((uchar)((w >> 8) & 255)), p2 = p1 + ig_val<T, SQ>((uchar)((w >> 16) & 255)),
+          p3 = p2 + ig_val<T, SQ>((uchar)(w >> 24));
+        T tot = p3;                                                 // inclusive scan of the lane totals
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) { const T up = ig_shfl_up<T>(tot, d); if (lane >= d) tot += up; }
+        const T base = carry + (tot - p3);                          // everything left of this lane's 4 pixels
+        if (x + 4 <= W) { o[x] = base + p0; o[x + 1] = base + p1; o[x + 2] = base + p2; o[x + 3] = base + p3; }
+        else {
+            if (x < W) o[x] = base + p0;
+            if (x + 1 < W) o[x + 1] = base + p1;
+            if (x + 2 < W) o[x + 2] = base + p2;
+        }
+        carry += ig_shfl<T>(tot, 31);
+    }
 }
 
 template <typename T>
-__global__ void __launch_bounds__(256) integral_h2_kernel(T* cs, IgDims g, int frames)
+__global__ void __launch_bounds__(128) integral_cols_kernel(Img out, int W, int H)
 {
-    const int r = blockIdx.x * blockDim.x + threadIdx.x;            // row index over all frames
-    if (r >= g.H * frames) return;
-    T* p = cs + (size_t)r * g.NC;
+    const int x = blockIdx.x * 128 + threadIdx.x, f = blockIdx.y;
+    if (x > W) return;
     T run = 0;
-    for (int c = 0; c < g.NC; c++) { const T v = p[c]; p[c] = run; run += v; }
+    int y = 1;
+    for (; y + 8 <= H + 1; y += 8) {
+        T v[8];
+#pragma unroll
+        for (int i = 0; i < 8; i++) v[i] = out.row<T>(f, y + i)[x];
+#pragma unroll
+        for (int i = 0; i < 8; i++) { run += v[i]; out.row<T>(f, y + i)[x] = run; }
+    }
+    for (; y <= H; y++) { T* p = out.row<T>(f, y) + x; run += *p; *p = run; }
 }
 
 template <typename T, bool SQ>
-__global__ void __launch_bounds__(256) integral_h3_kernel(Img src, Img out, const T* cs, IgDims g)
+int integral_launch(const Img& s, const Img& o, cudaStream_t st)
 {
-    const int c = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y, f = blockIdx.z;
-    if (c >= g.NC) return;
-    const uchar* s = src.row<uchar>(f, y) + c * IG_CHUNK;
-    const int n = min((int)IG_CHUNK, g.W - c * IG_CHUNK);
-    T* o = out.row<T>(f, y + 1) + 1 + c * IG_CHUNK;
-    T run = cs[((size_t)f * g.H + y) * g.NC + c];
-    for (int i = 0; i < n; i++) { run += ig_val<T, SQ>(s[i]); o[i] = run; }
-    if (c == 0) out.row<T>(f, y + 1)[0] = 0;                        // first column
-    if (y == 0) {                                                   // first row
-        T* z = out.row<T>(f, 0) + 1 + c * IG_CHUNK;
-        for (int i = 0; i < n; i++) z[i] = 0;
-        if (c == 0) out.row<T>(f, 0)[0] = 0;
-    }
-}
-
-template <typename T>
-__global__ void __launch_bounds__(256) integral_v1_kernel(Img out, T* bs, IgDims g)
-{
-    const int x = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y, f = blockIdx.z;
-    if (x >= g.W) return;
-    const int y0 = b * IG_ROWS, y1 = min(y0 + (int)IG_ROWS, g.H);
-    T acc = 0;
-    for (int y = y0; y < y1; y++) acc += out.row<T>(f, y + 1)[x + 1];
-    bs[((size_t)f * g.NB + b) * g.W + x] = acc;
-}
-
-template <typename T>
-__global__ void __launch_bounds__(256) integral_v2_kernel(T* bs, IgDims g)
-{
-    const int x = blockIdx.x * blockDim.x + threadIdx.x, f = blockIdx.z;
-    if (x >= g.W) return;
-    T* p = bs + (size_t)f * g.NB * g.W + x;
-    T run = 0;
-    for (int b = 0; b < g.NB; b++) { const T v = p[(size_t)b * g.W]; p[(size_t)b * g.W] = run; run += v; }
-}
-
-template <typename T>
-__global__ void __launch_bounds__(256) integral_v3_kernel(Img out, const T* bs, IgDims g)
-{
-    const int x = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y, f = blockIdx.z;
-    if (x >= g.W) return;
-    const int y0 = b * IG_ROWS, y1 = min(y0 + (int)IG_ROWS, g.H);
-    T run = bs[((size_t)f * g.NB + b) * g.W + x];
-    for (int y = y0; y < y1; y++) { T* o = out.row<T>(f, y + 1) + x + 1; run += *o; *o = run; }
-}
-
-template <typename T, bool SQ>
-int integral_run(const Img& s, const Img& o, cudaStream_t st)
-{
-    IgDims g;
-    g.W = s.cols; g.H = s.rows; g.NC = (int)div_up((unsigned)g.W, IG_CHUNK); g.NB = (int)div_up((unsigned)g.H, IG_ROWS);
-    const int frames = s.frames;
-#ifndef B200CV_HOST_EMULATION
-    {
-        // second version (integral_scan.cu): two kernels with warp scans; B200CV_INTEGRAL_PATH=v1 keeps the six map-only kernels below
-        const char* path = getenv("B200CV_INTEGRAL_PATH");
-        if (!(path && !strcmp(path, "v1"))) return integral_scan_run(s, o, SQ ? 1 : 0, st);
-    }
-#endif
-    T* scratch = nullptr;
-    const size_t ncs = (size_t)frames * g.H * g.NC, nbs = (size_t)frames * g.NB * g.W;
-    B200_CUDA(cudaMallocAsync((void**)&scratch, sizeof(T) * (ncs + nbs), st));
-    T* cs = scratch; T* bs = scratch + ncs;
-    const dim3 block(256);
-    {
-        const dim3 grid(div_up((unsigned)g.NC, 256), (unsigned)g.H, (unsigned)frames);
-        integral_h1_kernel<T, SQ><<<grid, block, 0, st>>>(s, cs, g);
-    }
-    {
-        const dim3 grid(div_up((unsigned)(g.H * frames), 256));
-        integral_h2_kernel<T><<<grid, block, 0, st>>>(cs, g, frames);
-    }
-    {
-        const dim3 grid(div_up((unsigned)g.NC, 256), (unsigned)g.H, (unsigned)frames);
-        integral_h3_kernel<T, SQ><<<grid, block, 0, st>>>(s, o, cs, g);
-    }
-    {
-        const dim3 grid(div_up((unsigned)g.W, 256), (unsigned)g.NB, (unsigned)frames);
-        integral_v1_kernel<T><<<grid, block, 0, st>>>(o, bs, g);
-    }
-    {
-        const dim3 grid(div_up((unsigned)g.W, 256), 1, (unsigned)frames);
-        integral_v2_kernel<T><<<grid, block, 0, st>>>(bs, g);
-    }
-    {
-        const dim3 grid(div_up((unsigned)g.W, 256), (unsigned)g.NB, (unsigned)frames);
-        integral_v3_kernel<T><<<grid, block, 0, st>>>(o, bs, g);
-    }
+    const int W = s.cols, H = s.rows, frames = s.frames;
+    const dim3 gr(div_up((unsigned)H, 8), (unsigned)frames), gc(div_up((unsigned)W + 1, 128), (unsigned)frames);
+    integral_rows_kernel<T, SQ><<<gr, 256, 0, st>>>(s, o, W, H);
+    integral_cols_kernel<T><<<gc, 128, 0, st>>>(o, W, H);
     const cudaError_t e = cudaGetLastError();
-    count_launch(6);
-    cudaFreeAsync(scratch, st);
+    count_launch(2);
     if (e != cudaSuccess) return cuda_fail(e, "kernel launch", __FILE__, __LINE__);
     return B200CV_OK;
 }
@@ -158,13 +114,13 @@ int integral_impl(const b200cvMat* src, const b200cvMat* sum, const b200cvMat* s
     Img s = make_img(src), o = make_img(sum);
     B200_REQUIRE(s.frames == o.frames, "src/dst batch mismatch");
     if (s.rows >= 65535 || s.frames >= 65536 || (size_t)s.rows * s.frames >= (1u << 31)) return B200CV_NOT_IMPLEMENTED;
-    int rc = integral_run<int, false>(s, o, st);
+    int rc = integral_launch<int, false>(s, o, st);
     if (rc || !sqsum || !sqsum->data) return rc;
     if (sqsum->type != B200CV_MAKETYPE(B200CV_64F, 1)) return B200CV_NOT_IMPLEMENTED;
     B200_REQUIRE(sqsum->cols == src->cols + 1 && sqsum->rows == src->rows + 1, "integral: sqsum must be (width + 1) x (height + 1)");
     Img q = make_img(sqsum);
     B200_REQUIRE(s.frames == q.frames, "src/dst batch mismatch");
-    return integral_run<double, true>(s, q, st);
+    return integral_launch<double, true>(s, q, st);
 }
 
 }  // namespace b200cv

@@ -725,13 +725,6 @@ int b200cv::gaussian_blur_impl(const b200cvMat* src, const b200cvMat* dst, int k
         B200_REQUIRE(src->cols == dst->cols && src->rows == dst->rows, "src/dst size mismatch");
         if (b < 0 || b > B200CV_BORDER_REFLECT_101) return B200CV_NOT_IMPLEMENTED;
         std::vector<long long> lx(fx.begin(), fx.end()), ly(fy.begin(), fy.end());
-        {   // second version: separable and tiled (gauss_u16_sep.cu); B200CV_GAUSS_U16_PATH=v1 keeps the direct window kernel
-            const char* path = getenv("B200CV_GAUSS_U16_PATH");
-            if (!(path && !strcmp(path, "v1"))) {
-                const int frc = gauss_u16_sep_impl(s, d, B200CV_CN(src->type), lx.data(), kw, ly.data(), kh, b, as_stream(stream));
-                if (frc != B200CV_NOT_IMPLEMENTED) return frc;
-            }
-        }
         return gauss_u16_impl(s, d, B200CV_CN(src->type), lx.data(), kw, ly.data(), kh, b, as_stream(stream));
     }
     if (depth == B200CV_8U) {

@@ -1,8 +1,8 @@
-// sift_desc_warp.cu -- SIFT descriptors, second version of sift_detect.cu's thread-per-keypoint kernel (1.4 KB of local memory per thread and a
-// serial loop over the (2 r + 1)^2 samples of the patch: a few thousand threads, each running ~10^5 dependent instructions).
-// Here a WARP owns a keypoint: the samples of the patch are dealt out to the lanes, the 6 x 6 x 10 tri-linear histogram lives in shared
-// memory.  Float atomics would make the sum depend on the order the lanes happen to arrive in (run-to-run differences of +-1 in a descriptor
-// byte); instead every contribution is added as a 64-bit fixed-point integer (2^-24 units: integer addition is associative, so the histogram
+// sift_desc_warp.cu -- SIFT descriptors of the keypoints sift_detect.cu found.  A WARP owns a keypoint: the (2 r + 1)^2 samples of the patch
+// are dealt out to the lanes (a thread per keypoint would be a few thousand threads, each running ~10^5 dependent instructions), and the
+// 6 x 6 x 10 tri-linear histogram lives in shared memory.  Float atomics would make the sum depend on the order the lanes happen to arrive
+// in (run-to-run differences of +-1 in a descriptor byte); instead every contribution is added as a 64-bit fixed-point integer
+// (2^-24 units: integer addition is associative, so the histogram
 // is the same whatever the order, and the quantisation -- 6e-8 per contribution against bin totals of 10..1000 -- is below the float
 // rounding of the reference's own sequential accumulation).  Same arithmetic otherwise: calcSIFTDescriptor, sift.simd.hpp:709-1035
 // (fastAtan2's polynomial, exp, the tri-linear split, clipping at 0.2 |h|, scaling to 512, saturation to bytes).

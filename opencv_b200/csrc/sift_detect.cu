@@ -12,10 +12,10 @@
 // Parity is by tolerance, as for the port (oracle/port/port_features.c: the reference's objects are FMA-contracted and use OpenCV's own
 // exp / atan2 approximations): keypoints agree to ~1e-4 px apart from borderline accept / reject decisions, descriptor bytes to +-1.
 // fastAtan2's polynomial (mathfuncs_core.simd.hpp:52-72) is reproduced because its 0.3-degree error moves samples between bins.
-// Three kernels, one thread per DoG pixel / candidate / keypoint; candidates and keypoints are appended with atomics and the final order
-// is fixed by the reference's own sort (KeyPoint12_LessThan) on the host, where the reference also does it.
+// Two kernels, one thread per DoG pixel / candidate; candidates and keypoints are appended with atomics and the final order is fixed by
+// the reference's own sort (KeyPoint12_LessThan) on the host, where the reference also does it.  The descriptors of the sorted keypoints
+// are computed by sift_desc_warp.cu, a warp per keypoint.
 #include <math.h>
-#include <stdlib.h>
 #include <string.h>
 #include <algorithm>
 #include <vector>
@@ -165,80 +165,6 @@ __global__ void __launch_bounds__(128) sift_refine_kernel(SiftPyr p, const SiftC
     }
 }
 
-// ---- 3. descriptors: one thread per keypoint (keypoints in image coordinates, i.e. after the first-octave rescaling) ----------------------
-__global__ void __launch_bounds__(64) sift_descriptor_kernel(SiftPyr p, int first_octave, const SiftKp* kps, int nkp, float* desc)
-{
-    const int q = blockIdx.x * blockDim.x + threadIdx.x;
-    if (q >= nkp) return;
-    enum { d = 4, n = 8 };
-    const SiftKp k = kps[q];
-    int octave = k.octave & 255;
-    const int layer = (k.octave >> 8) & 255;
-    octave = octave < 128 ? octave : (-128 | octave);
-    const float scale = octave >= 0 ? 1.f / (1 << octave) : (float)(1 << -octave);
-    const int oi = octave - first_octave;
-    float* out = desc + (size_t)q * 128;
-    if (oi < 0 || oi >= p.n_oct || layer > p.nl + 2) { for (int e = 0; e < 128; e++) out[e] = 0.f; return; }
-    const int cols = p.w[oi], rows = p.h[oi];
-    const float* img = p.gauss + p.goff[oi] + (size_t)layer * cols * rows;
-    const float size = k.size * scale, ptx = k.x * scale, pty = k.y * scale;
-    float ori = 360.f - k.angle;
-    if (fabsf(ori - 360.f) < 1.1920929e-07f) ori = 0.f;
-    const float scl = size * 0.5f;
-    const int px = __float2int_rn(ptx), py = __float2int_rn(pty);
-    float cos_t = cosf(ori * (float)(3.1415926535897932384626433832795 / 180)), sin_t = sinf(ori * (float)(3.1415926535897932384626433832795 / 180));
-    const float bins_per_rad = n / 360.f, exp_scale = -1.f / (d * d * 0.5f), hist_width = 3.f * scl;
-    int radius = __float2int_rn(hist_width * 1.4142135623730951f * (d + 1) * 0.5f);
-    radius = min(radius, (int)sqrt((double)cols * cols + (double)rows * rows));
-    cos_t /= hist_width; sin_t /= hist_width;
-    float hist[(d + 2) * (d + 2) * (n + 2)];
-    for (int i = 0; i < (d + 2) * (d + 2) * (n + 2); i++) hist[i] = 0.f;
-    for (int i = -radius; i <= radius; i++)
-        for (int j = -radius; j <= radius; j++) {
-            const float c_rot = j * cos_t - i * sin_t, r_rot = j * sin_t + i * cos_t;
-            float rbin = r_rot + d / 2 - 0.5f, cbin = c_rot + d / 2 - 0.5f;
-            const int r = py + i, c = px + j;
-            if (!(rbin > -1 && rbin < d && cbin > -1 && cbin < d && r > 0 && r < rows - 1 && c > 0 && c < cols - 1)) continue;
-            const float dx = img[(size_t)r * cols + c + 1] - img[(size_t)r * cols + c - 1];
-            const float dy = img[(size_t)(r - 1) * cols + c] - img[(size_t)(r + 1) * cols + c];
-            const float w = expf((c_rot * c_rot + r_rot * r_rot) * exp_scale);
-            float obin = (fast_atan2_deg(dy, dx) - ori) * bins_per_rad;
-            const float mag = sqrtf(dx * dx + dy * dy) * w;
-            const int r0 = (int)floorf(rbin), c0 = (int)floorf(cbin);
-            int o0 = (int)floorf(obin);
-            rbin -= r0; cbin -= c0; obin -= o0;
-            if (o0 < 0) o0 += n;
-            if (o0 >= n) o0 -= n;
-            // tri-linear split: the upper share of each axis is weight * fraction, the lower share the remainder (sift.simd.hpp:864-882)
-            const int idx = ((r0 + 1) * (d + 2) + c0 + 1) * (n + 2) + o0;
-            const float up_r = mag * rbin;
-#pragma unroll
-            for (int ri = 0; ri < 2; ri++) {
-                const float w_r = ri ? up_r : mag - up_r;
-                const float up_c = w_r * cbin;
-#pragma unroll
-                for (int ci = 0; ci < 2; ci++) {
-                    const float w_c = ci ? up_c : w_r - up_c;
-                    const float up_o = w_c * obin;
-                    float* cell = hist + idx + ri * (d + 2) * (n + 2) + ci * (n + 2);
-                    cell[0] += w_c - up_o; cell[1] += up_o;
-                }
-            }
-        }
-    float nrm2 = 0;
-    for (int i = 0; i < d; i++)
-        for (int j = 0; j < d; j++) {
-            const int idx = ((i + 1) * (d + 2) + (j + 1)) * (n + 2);
-            hist[idx] += hist[idx + n]; hist[idx + 1] += hist[idx + n + 1];
-            for (int e = 0; e < n; e++) { const float v = hist[idx + e]; out[(i * d + j) * n + e] = v; nrm2 += v * v; }
-        }
-    const float thr = sqrtf(nrm2) * 0.2f;
-    nrm2 = 0;
-    for (int e = 0; e < 128; e++) { const float v = fminf(out[e], thr); out[e] = v; nrm2 += v * v; }
-    nrm2 = 512.f / fmaxf(sqrtf(nrm2), 1.1920929e-07f);
-    for (int e = 0; e < 128; e++) out[e] = (float)sat_u8(__float2int_rn(out[e] * nrm2));
-}
-
 struct KpLess {      // KeyPoint12_LessThan, features2d/src/keypoint.cpp:253-271 (class_id is always -1)
     bool operator()(const SiftKp& a, const SiftKp& b) const
     {
@@ -350,31 +276,19 @@ int sift_detect_impl(const float* gauss, const float* dog, const int* dims, int 
         o6[0] = hk[j].x; o6[1] = hk[j].y; o6[2] = hk[j].size; o6[3] = hk[j].angle; o6[4] = hk[j].response; memcpy(o6 + 5, &hk[j].octave, 4);
     }
     int rc = B200CV_OK;
+#ifndef B200CV_HOST_EMULATION
     if (desc_host && nret) {
         // the sorted keypoints go back up (they fit in the keypoint buffer), descriptors come down
         float* ddesc = nullptr;
         ce = cudaMallocAsync((void**)&ddesc, sizeof(float) * 128 * nret, st);
         if (ce == cudaSuccess) ce = cudaMemcpyAsync(kps, hk.data(), sizeof(SiftKp) * nret, cudaMemcpyHostToDevice, st);
-        bool warp_path = false;
-#ifndef B200CV_HOST_EMULATION
-        {   // second version: a warp per keypoint (sift_desc_warp.cu); B200CV_SIFT_DESC_PATH=v1 keeps the thread-per-keypoint kernel below
-            const char* path = getenv("B200CV_SIFT_DESC_PATH");
-            warp_path = !(path && !strcmp(path, "v1"));
-            if (ce == cudaSuccess && warp_path && sift_descriptors_warp(p, first_octave, kps, (int)nret, ddesc, st) != B200CV_OK) ce = cudaErrorUnknown;
-        }
-#endif
-        if (ce == cudaSuccess && !warp_path) {
-            const dim3 block(64);
-            const dim3 grid(div_up((unsigned)nret, 64));
-            sift_descriptor_kernel<<<grid, block, 0, st>>>(p, first_octave, kps, (int)nret, ddesc);
-            count_launch();
-            ce = cudaGetLastError();
-        }
+        if (ce == cudaSuccess && sift_descriptors_warp(p, first_octave, kps, (int)nret, ddesc, st) != B200CV_OK) ce = cudaErrorUnknown;
         if (ce == cudaSuccess) ce = cudaMemcpyAsync(desc_host, ddesc, sizeof(float) * 128 * nret, cudaMemcpyDeviceToHost, st);
         if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
         if (ddesc) cudaFreeAsync(ddesc, st);
         if (ce != cudaSuccess) rc = cuda_fail(ce, "sift descriptors", __FILE__, __LINE__);
     }
+#endif
     cudaFreeAsync(scratch, st);
     return rc;
 }

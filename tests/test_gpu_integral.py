@@ -10,7 +10,7 @@ from util import assert_exact, cpu, gpu
 pytestmark = [pytest.mark.gpu]
 
 
-@pytest.mark.parametrize("size", [(1, 1), (5, 7), (17, 15), (33, 65), (240, 321), (1080, 1920), (2160, 3840)])
+@pytest.mark.parametrize("size", [(1, 1), (5, 7), (16, 16), (17, 15), (33, 65), (100, 257), (240, 321), (1080, 1920), (2160, 3840)])
 def test_integral(cvb, oracle, rng, size):
     img = rng.integers(0, 256, size, dtype=np.uint8)
     ws, wq = oracle.integral(img, True)
@@ -42,13 +42,13 @@ def test_integral_batch_host_and_hal(cvb, oracle, rng):
     assert s[300, 400] - s[100, 400] - s[300, 200] + s[100, 200] == int(img[100:300, 200:400].sum(dtype=np.int64))
 
 
-def test_integral_first_version_still_agrees(cvb, oracle, rng, monkeypatch):
-    """B200CV_INTEGRAL_PATH=v1: the six map-only kernels (the ones the host emulation runs) against the warp-scan kernels and the oracle"""
-    img = rng.integers(0, 256, (3, 333, 517, 1), dtype=np.uint8)
-    s2, q2 = cvb.integral(gpu(img), with_sqsum=True)
-    monkeypatch.setenv("B200CV_INTEGRAL_PATH", "v1")
-    s1, q1 = cvb.integral(gpu(img), with_sqsum=True)
-    monkeypatch.delenv("B200CV_INTEGRAL_PATH")
-    assert_exact(cpu(s2), cpu(s1), "integral sum: scan kernels vs map-only kernels")
-    assert_exact(cpu(q2), cpu(q1), "integral sqsum: scan kernels vs map-only kernels")
-    assert_exact(cpu(s2)[1, :, :, 0], oracle.integral(img[1, :, :, 0]), "integral sum vs oracle")
+def test_integral_batch_every_frame(cvb, oracle, rng):
+    for shape in ((3, 333, 517, 1), (3, 40, 50, 1)):
+        batch = rng.integers(0, 256, shape, dtype=np.uint8)
+        gs, gq = cvb.integral(gpu(batch), with_sqsum=True)
+        gs, gq = cpu(gs), cpu(gq)
+        assert_exact(cpu(cvb.integral(gpu(batch))), gs, "integral sum only %s" % (shape,))
+        for f in range(shape[0]):
+            ws, wq = oracle.integral(batch[f, :, :, 0], True)
+            assert_exact(gs[f, :, :, 0], ws, "integral sum %s frame %d" % (shape, f))
+            assert_exact(gq[f, :, :, 0], wq, "integral sqsum %s frame %d" % (shape, f))

@@ -9,8 +9,8 @@ port = Oracle("port")
 rng = np.random.default_rng(int(time.time()))
 def fx(f):  # unwrap pytest fixture
     return f.__wrapped__() if hasattr(f, "__wrapped__") else f()
-two = fx(T.two_plane_emu); mtm = fx(T.mtmask_emu); g16 = T.gauss16_emu.__wrapped__(port)
-yuv = fx(T.yuv_emu); area = fx(T.area_emu); exact = fx(T.exact_emu); lz = fx(T.lanczos_emu); bayer = fx(T.bayer_emu); integ = fx(T.integral_emu); lab = fx(T.lab_emu)
+two = fx(T.two_plane_emu); mtm = fx(T.mtmask_emu)
+yuv = fx(T.yuv_emu); area = fx(T.area_emu); exact = fx(T.exact_emu); lz = fx(T.lanczos_emu); bayer = fx(T.bayer_emu); lab = fx(T.lab_emu)
 t0 = time.time(); n = 0
 while time.time() - t0 < 150:
     h = int(rng.integers(1, 40)) * 2; w = int(rng.integers(1, 60)) * 2
@@ -35,10 +35,9 @@ while time.time() - t0 < 150:
                 assert np.array_equal(area(im, (dw, dh)), port.resize(im, (dw, dh), 3)), ("area", im.dtype, sh, sw, dh, dw, cn)
     g = rng.integers(0, 256, (max(sh, 3), max(sw, 3)), dtype=np.uint8)
     code = int(rng.choice([46, 47, 48, 49, 139, 140, 141, 142])); assert np.array_equal(bayer(g, code), port.cvtColorYUV(g, code)), ("bayer", g.shape, code)
-    ws, wq = port.integral(g, True); gs, gq = integ(g, True); assert np.array_equal(gs, ws) and np.array_equal(gq, wq), ("integral", g.shape)
     c3 = rng.integers(0, 256, (sh, sw, 3), dtype=np.uint8); code = int(rng.choice([32,33,34,35,44,45,74,75,56,57,78,79]))
     assert np.array_equal(lab(c3, code), port.cvtColorLab(c3, code)), ("lab", code)
-    # two-plane NV12 / NV21, masked matchTemplate, 16-bit GaussianBlur
+    # two-plane NV12 / NV21, masked matchTemplate
     yp = rng.integers(0, 256, (h, w), dtype=np.uint8); uvp = rng.integers(0, 256, (h // 2, w // 2, 2), dtype=np.uint8); code = int(rng.integers(90, 98))
     assert np.array_equal(two(yp, uvp, code), port.cvtColorTwoPlane(yp, uvp, code)), ("two-plane", h, w, code)
     ih, iw = int(rng.integers(8, 40)), int(rng.integers(8, 40)); th, tw = int(rng.integers(1, ih + 1)), int(rng.integers(1, iw + 1))
@@ -48,8 +47,5 @@ while time.time() - t0 < 150:
         meth = int(rng.integers(0, 6))
         a, b2 = mtm(im, tt, mk, meth), port.matchTemplateMasked(im, tt, meth, mk)
         assert np.array_equal(a, b2, equal_nan=True), ("masked MT", ih, iw, th, tw, meth)
-    if sh > 1 and sw > 1:
-        u16 = rng.integers(0, 65536, shape, dtype=np.uint16); k = int(rng.choice([3, 5, 7, 9, 13])); sg = float(rng.choice([0, 0.8, 2.1])); bd = int(rng.choice([0, 1, 2, 3, 4]))
-        assert np.array_equal(g16(u16, k, sg, bd), port.GaussianBlur(u16, (k, k), sg, sg, bd)), ("gauss u16", shape, k, sg, bd)
     n += 1
 print("fuzz iterations", n, "all equal")
