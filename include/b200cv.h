@@ -92,6 +92,19 @@ extern "C" {
 #define B200CV_TM_CCOEFF 4
 #define B200CV_TM_CCOEFF_NORMED 5
 
+/* cv::DistanceTypes and cv::DistanceTransformMasks (imgproc.hpp) */
+#define B200CV_DIST_USER (-1)
+#define B200CV_DIST_L1 1
+#define B200CV_DIST_L2 2
+#define B200CV_DIST_C 3
+#define B200CV_DIST_L12 4
+#define B200CV_DIST_FAIR 5
+#define B200CV_DIST_WELSCH 6
+#define B200CV_DIST_HUBER 7
+#define B200CV_DIST_MASK_PRECISE 0
+#define B200CV_DIST_MASK_3 3
+#define B200CV_DIST_MASK_5 5
+
 /* A (batch of) device image(s).  frames<=1 means a single frame (frame_step ignored). */
 typedef struct b200cvMat {
     void*  data;        /* device pointer to pixel (0,0) of frame 0 */
@@ -235,6 +248,17 @@ B200CV_API int b200cv_canny(const b200cvMat* src, const b200cvMat* dst, double t
                             int l2gradient, void* stream);
 B200CV_API int b200cv_canny_derivs(const b200cvMat* dx, const b200cvMat* dy, const b200cvMat* dst, double threshold1, double threshold2,
                                    int l2gradient, void* stream);
+/* replaces cv::distanceTransform(src, dst, distanceType, maskSize, dstType) (imgproc.hpp; distransform.cpp), bit-exact.  src: 8UC1.
+ * dst 32FC1 of the source size: DIST_C and DIST_L1 run the 3x3 chamfer whatever the mask (which must still be 0, 3 or 5), DIST_L2 the
+ * 3x3 (0.955, 1.3693) or 5x5 (1, 1.4, 2.1969) chamfer in 16.16 fixed point, and mask 0 (B200CV_DIST_MASK_PRECISE) the exact Euclidean
+ * transform for every type but C and L1, as the reference does (so DIST_L12, DIST_FAIR, DIST_WELSCH, DIST_HUBER and DIST_USER run it
+ * too).  An image without a zero pixel gives the chamfer's DIST_MAX / 65536 everywhere.
+ * dst 8UC1: the 8-bit L1 call (dstType CV_8U), min(255, city-block distance); DIST_L1 only, mask not checked; src == dst allowed.
+ * Chamfer: one launch, one CTA per frame, 2 * H dependent row steps; scratch of 4 B per pixel per frame from the stream-ordered pool.
+ * Precise: two launches; rows wider than 19 370 pixels keep the envelope stacks in a scratch of 12 B per column per resident warp
+ * (narrower ones in shared memory).  Nothing synchronises the host.  distanceTransformWithLabels is not offered.
+ * src not 8UC1, a mask or type the reference refuses, a dst of another type or size, W * H >= 2^31: B200CV_ERR_BAD_ARG, dst untouched. */
+B200CV_API int b200cv_distance_transform(const b200cvMat* src, const b200cvMat* dst, int distance_type, int mask_size, void* stream);
 /* SIFT Gaussian pyramid + DoG (features2d/src/sift.dispatch.cpp:176-310).
  * src: 8UC1 batch.  gauss / dog: device float buffers, per frame packed image after image, octave-major
  * (n_octaves*(n_layers+3) Gaussian images, n_octaves*(n_layers+2) DoG images); per-frame strides in floats.

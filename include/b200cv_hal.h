@@ -149,6 +149,9 @@ B200CV_API int b200cv_host_corner_harris(const b200cvMat* src, const b200cvMat* 
 B200CV_API int b200cv_host_corner_min_eigen_val(const b200cvMat* src, const b200cvMat* dst, int block_size, int ksize, int border);
 /* cv::Canny over host frames; thresholds and aperture as b200cv_canny takes them */
 B200CV_API int b200cv_host_canny(const b200cvMat* src, const b200cvMat* dst, double threshold1, double threshold2, int aperture_size, int l2gradient);
+/* cv::distanceTransform over host frames; arguments as b200cv_distance_transform takes them (the type of dst selects the 8-bit L1 call).
+ * The reference has no HAL hook for it, so there is no hal_ni_* counterpart. */
+B200CV_API int b200cv_host_distance_transform(const b200cvMat* src, const b200cvMat* dst, int distance_type, int mask_size);
 
 #ifdef __cplusplus
 }

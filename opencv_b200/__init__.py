@@ -4,7 +4,7 @@ The functions mirror the cv2 / cv:: names and argument meaning of the reference
 (modules/imgproc/include/opencv2/imgproc.hpp) for the calls on the hot path:
 
     GaussianBlur, sepFilter2D, filter2D, Sobel, resize, warpAffine, warpPerspective, cvtColor,
-    matchTemplate, cornerHarris, cornerMinEigenVal, goodFeaturesToTrack, Canny, sift_pyramid
+    matchTemplate, cornerHarris, cornerMinEigenVal, goodFeaturesToTrack, Canny, distanceTransform, sift_pyramid
 
 Inputs are torch CUDA tensors laid out like a cv::Mat -- (H, W) or (H, W, C), or a batch
 (N, H, W[, C]) of independent frames -- and go to the device C ABI (include/b200cv.h) without a
@@ -31,6 +31,9 @@ INTER_NEAREST, INTER_LINEAR, INTER_CUBIC, INTER_AREA = 0, 1, 2, 3
 INTER_LANCZOS4, INTER_LINEAR_EXACT, INTER_NEAREST_EXACT = 4, 5, 6
 WARP_INVERSE_MAP = 16
 TM_SQDIFF, TM_SQDIFF_NORMED, TM_CCORR, TM_CCORR_NORMED, TM_CCOEFF, TM_CCOEFF_NORMED = range(6)
+# cv::DistanceTypes and cv::DistanceTransformMasks
+DIST_USER, DIST_L1, DIST_L2, DIST_C, DIST_L12, DIST_FAIR, DIST_WELSCH, DIST_HUBER = -1, 1, 2, 3, 4, 5, 6, 7
+DIST_MASK_3, DIST_MASK_5, DIST_MASK_PRECISE = 3, 5, 0
 COLOR_BGR2BGRA, COLOR_BGRA2BGR, COLOR_BGR2RGBA, COLOR_RGBA2BGR, COLOR_BGR2RGB, COLOR_BGRA2RGBA = range(6)
 COLOR_RGB2BGRA, COLOR_BGRA2RGB, COLOR_RGB2BGR, COLOR_RGBA2BGRA = COLOR_BGR2RGBA, COLOR_RGBA2BGR, COLOR_BGR2RGB, COLOR_BGRA2RGBA
 COLOR_BGR2GRAY, COLOR_RGB2GRAY, COLOR_GRAY2BGR, COLOR_GRAY2BGRA, COLOR_BGRA2GRAY, COLOR_RGBA2GRAY = 6, 7, 8, 9, 10, 11
@@ -520,6 +523,24 @@ def _canny_derivs(dx, dy, threshold1, threshold2, edges=None, L2gradient=False, 
     _check(lib().b200cv_canny_derivs(ctypes.byref(mx), ctypes.byref(my), ctypes.byref(md), ctypes.c_double(threshold1), ctypes.c_double(threshold2),
                                      int(bool(L2gradient)), _stream_ptr(stream)), "Canny")
     return edges
+
+
+def distanceTransform(src, distanceType, maskSize, dst=None, dstType=CV_32F, stream=None):
+    """cv::distanceTransform(src, distanceType, maskSize, dst, dstType) over an 8UC1 image or (N, H, W, 1) batch: the distance of every
+    pixel to the nearest zero pixel.  The result is 8UC1 for DIST_L1 with dstType CV_8U (the saturating city-block call, which may run
+    in place: dst=src) and 32FC1 otherwise, as in the reference.  DIST_C and DIST_L1 always use the 3x3 mask; maskSize 0
+    (DIST_MASK_PRECISE) gives the exact Euclidean distance for every other type."""
+    if not _is_torch(src):
+        from . import hal
+        return hal.distanceTransform(src, distanceType, maskSize, dst, dstType)
+    import torch
+    if dst is None:
+        u8 = distanceType == DIST_L1 and dstType == CV_8U
+        dst = _new(src, dtype=torch.uint8 if u8 else torch.float32, channels=1)
+    ms, md = _pair(src, dst)
+    _check(lib().b200cv_distance_transform(ctypes.byref(ms), ctypes.byref(md), int(distanceType), int(maskSize), _stream_ptr(stream)),
+           "distanceTransform")
+    return dst
 
 
 def goodFeaturesToTrack(image, maxCorners, qualityLevel, minDistance, blockSize=3, gradientSize=3, useHarrisDetector=False, k=0.04,

@@ -198,6 +198,8 @@ extern "C" int b200cv_host_corner_min_eigen_val(const b200cvMat* s, const b200cv
 { return host_pipeline(s, d, [=](const b200cvMat* a, const b200cvMat* b, void* st) { return b200cv_corner_min_eigen_val(a, b, bs, ks, border, st); }); }
 extern "C" int b200cv_host_canny(const b200cvMat* s, const b200cvMat* d, double t1, double t2, int aperture, int l2)
 { return host_pipeline(s, d, [=](const b200cvMat* a, const b200cvMat* b, void* st) { return b200cv_canny(a, b, t1, t2, aperture, l2, st); }); }
+extern "C" int b200cv_host_distance_transform(const b200cvMat* s, const b200cvMat* d, int distance_type, int mask_size)
+{ return host_pipeline(s, d, [=](const b200cvMat* a, const b200cvMat* b, void* st) { return b200cv_distance_transform(a, b, distance_type, mask_size, st); }); }
 
 extern "C" int b200cv_host_match_template(const b200cvMat* image, const b200cvMat* templ, const b200cvMat* result, int method)
 {

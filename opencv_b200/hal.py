@@ -104,6 +104,16 @@ def Sobel(src, ddepth, dx, dy, ksize=3, scale=1.0, delta=0.0, borderType=BORDER_
     return dst
 
 
+def distanceTransform(src, distanceType, maskSize, dst=None, dstType=CV_32F):
+    """cv::distanceTransform over host 8UC1 arrays (b200cv_host_distance_transform): 8UC1 for DIST_L1 with dstType CV_8U, 32FC1
+    otherwise; dst=src runs the 8-bit L1 call in place."""
+    if dst is None:
+        dst = _new(src, dtype=np.uint8 if (distanceType == 1 and dstType == CV_8U) else np.float32, channels=1)
+    ms, md = describe(src), describe(dst)
+    _check(lib().b200cv_host_distance_transform(ctypes.byref(ms), ctypes.byref(md), int(distanceType), int(maskSize)), "distanceTransform")
+    return dst
+
+
 def Canny(*args, **kwargs):
     """cv::Canny over host arrays, both overloads: Canny(image, threshold1, threshold2, edges=None, apertureSize=3, L2gradient=False) and
     Canny(dx, dy, threshold1, threshold2, edges=None, L2gradient=False).  The image overload runs b200cv_host_canny; the derivative

@@ -6,7 +6,8 @@
 //                                               (createGaussianFilter(type, type, ksize, sigma) -> apply(src, dst, stream))
 //   b200cv::GaussianBlur, sepFilter2D, filter2D, Sobel, resize, warpAffine, warpPerspective, cvtColor, matchTemplate, cornerHarris,
 //   cornerMinEigenVal, goodFeaturesToTrack,     same argument order and meaning as imgproc.hpp:1544,1723,1702,1862,2422,2450,2482,3736,
-//   Canny                                       3916,1948,1921,2096,1889,1907, with a trailing Stream& like the cv::cuda:: functions
+//   Canny, distanceTransform                    3916,1948,1921,2096,1889,1907 and cv::distanceTransform, with a trailing Stream& like
+//                                               the cv::cuda:: functions
 // With -DB200CV_WITH_OPENCV (OpenCV headers on the include path) b200cv_opencv.hpp adds namespace b200cv::cuda: the same operations over
 // cv::InputArray / cv::OutputArray (cv::Mat, cv::cuda::GpuMat, cv::cuda::HostMem) with cv::cuda's Filter / Stream& shapes.
 // Errors: the C ABI status is turned into b200cv::Error (std::runtime_error); NOT_IMPLEMENTED is b200cv::NotImplemented.
@@ -203,6 +204,10 @@ inline void Canny(const GpuMat& image, GpuMat& edges, double threshold1, double 
 inline void Canny(const GpuMat& dx, const GpuMat& dy, GpuMat& edges, double threshold1, double threshold2, bool L2gradient = false, Stream& s = Stream::Null())
 { B200CV_DST(edges, dx, makeType(CV_8U, 1)); b200cvMat a = dx.desc(), b = dy.desc(), c = edges.desc();
   check(b200cv_canny_derivs(&a, &b, &c, threshold1, threshold2, L2gradient ? 1 : 0, s.cudaPtr()), "Canny"); }
+// cv::distanceTransform(src, dst, distanceType, maskSize, dstType): 8UC1 -> 32FC1, or 8UC1 for DIST_L1 with dstType CV_8U (src == dst allowed)
+inline void distanceTransform(const GpuMat& src, GpuMat& dst, int distanceType, int maskSize, int dstType = CV_32F, Stream& s = Stream::Null())
+{ B200CV_DST(dst, src, makeType(distanceType == B200CV_DIST_L1 && dstType == CV_8U ? CV_8U : CV_32F, 1)); b200cvMat a = src.desc(), b = dst.desc();
+  check(b200cv_distance_transform(&a, &b, distanceType, maskSize, s.cudaPtr()), "distanceTransform"); }
 inline void goodFeaturesToTrack(const GpuMat& image, std::vector<Point2f>& corners, int maxCorners, double qualityLevel, double minDistance, int blockSize = 3,
                                 int gradientSize = 3, bool useHarrisDetector = false, double k = 0.04, Stream& s = Stream::Null())
 { int cap = maxCorners > 0 ? maxCorners : image.rows * image.cols; std::vector<float> pts((size_t)2 * cap * image.frames); std::vector<int> cnt(image.frames);

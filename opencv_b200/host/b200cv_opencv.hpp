@@ -4,7 +4,7 @@
 //
 //   namespace b200cv::cuda   what a user of cv::cuda:: switches to (rename the namespace, keep the code): the reference signatures of
 //       GaussianBlur / sepFilter2D / filter2D / Sobel / resize / warpAffine / warpPerspective / cvtColor / matchTemplate / cornerHarris /
-//       cornerMinEigenVal / goodFeaturesToTrack / Canny (imgproc.hpp:1544,1723,1702,1862,2422,2450,2482,3736,3916,1948,1921,2096,1889,1907) + Stream&, and
+//       cornerMinEigenVal / goodFeaturesToTrack / Canny / distanceTransform (imgproc.hpp:1544,1723,1702,1862,2422,2450,2482,3736,3916,1948,1921,2096,1889,1907) + Stream&, and
 //       GFTTDetector (features2d/src/gftt.cpp), createGaussianFilter / createSeparableLinearFilter / createLinearFilter / createSobelFilter -> Ptr<Filter>, Filter::apply(InputArray,
 //       OutputArray, Stream&) -- the usage of samples/cpp/tutorial_code/gpu/gpu-basics-similarity/gpu-basics-similarity.cpp:392-404.
 //   Array kinds accepted (core/include/opencv2/core/mat.hpp:163-188):
@@ -269,6 +269,16 @@ inline void Canny(cv::InputArray image, cv::OutputArray edges, double threshold1
     const int l2 = L2gradient ? 1 : 0;
     check(a.device ? b200cv_canny(&a.m, &b.m, threshold1, threshold2, apertureSize, l2, s.cudaPtr())
                    : b200cv_host_canny(&a.m, &b.m, threshold1, threshold2, apertureSize, l2), "Canny");
+}
+// cv::distanceTransform(src, dst, distanceType, maskSize, dstType): the reference has no HAL hook for it, so a stock cv::distanceTransform
+// never reaches the library; call this instead.  8UC1 for DIST_L1 with dstType CV_8U (in place allowed), 32FC1 otherwise.
+inline void distanceTransform(cv::InputArray src, cv::OutputArray dst, int distanceType, int maskSize, int dstType = CV_32F, Stream& s = Stream::Null())
+{
+    Arr a = input(src, "distanceTransform");
+    const int t = distanceType == cv::DIST_L1 && dstType == CV_8U ? CV_8UC1 : CV_32FC1;
+    Arr b = output(dst, a.m.rows, a.m.cols, t, a.device, "distanceTransform");
+    check(a.device ? b200cv_distance_transform(&a.m, &b.m, distanceType, maskSize, s.cudaPtr())
+                   : b200cv_host_distance_transform(&a.m, &b.m, distanceType, maskSize), "distanceTransform");
 }
 // host derivatives are uploaded, the edges downloaded (there is no batched host path for this overload)
 inline void Canny(cv::InputArray dx, cv::InputArray dy, cv::OutputArray edges, double threshold1, double threshold2, bool L2gradient = false,
