@@ -174,6 +174,13 @@ B200CV_API int b200cv_filter2d(const b200cvMat* src, const b200cvMat* dst, const
 /* replaces cv::Sobel (imgproc.hpp:1862; deriv.cpp:414-465) for ksize 1/3/5/7 */
 B200CV_API int b200cv_sobel(const b200cvMat* src, const b200cvMat* dst, int dx, int dy, int ksize, double scale,
                             double delta, int border, void* stream);
+/* replaces cv::Laplacian(src, dst, ddepth, ksize, scale, delta, borderType) (imgproc.hpp; deriv.cpp:787-876), bit-exact.  dst's depth is
+ * ddepth: 8U -> 8U / 16S / 32F and 32F -> 32F, 1 to 4 channels; any other pair returns B200CV_NOT_IMPLEMENTED (16U / 16S sources and 64F
+ * destinations among them).  ksize 1 / 3 run filter2D with the reference's scaled 3x3 kernel; odd ksize 5..31 run one fused launch
+ * (two separable second derivatives, their sum and convertTo's scale and delta, no intermediate plane).  Any other ksize returns
+ * B200CV_ERR_BAD_ARG.  Borders CONSTANT (zero), REPLICATE, REFLECT, REFLECT_101, each with or without ISOLATED (a view has no parent,
+ * so ISOLATED changes nothing); WRAP returns B200CV_NOT_IMPLEMENTED.  src == dst is refused.  Batches: one launch for all frames. */
+B200CV_API int b200cv_laplacian(const b200cvMat* src, const b200cvMat* dst, int ksize, double scale, double delta, int border, void* stream);
 /* replaces cv::boxFilter / cv::blur (imgproc.hpp:1603, :1659; box_filter.dispatch.cpp:440-498).  dst depth picks ddepth:
  * 8U->8U, 8U->32F, 32F->32F; anchor (-1,-1) = centre; borders CONSTANT (zeros), REPLICATE, REFLECT, REFLECT_101; ksize <= 128x128. */
 B200CV_API int b200cv_box_filter(const b200cvMat* src, const b200cvMat* dst, int ksize_w, int ksize_h, int anchor_x, int anchor_y,

@@ -132,6 +132,7 @@ B200CV_API int b200cv_host_sep_filter2d(const b200cvMat* src, const b200cvMat* d
 B200CV_API int b200cv_host_filter2d(const b200cvMat* src, const b200cvMat* dst, const float* kernel, int kw, int kh, int anchor_x, int anchor_y,
                                     double delta, int border);
 B200CV_API int b200cv_host_sobel(const b200cvMat* src, const b200cvMat* dst, int dx, int dy, int ksize, double scale, double delta, int border);
+B200CV_API int b200cv_host_laplacian(const b200cvMat* src, const b200cvMat* dst, int ksize, double scale, double delta, int border);
 B200CV_API int b200cv_host_box_filter(const b200cvMat* src, const b200cvMat* dst, int ksize_w, int ksize_h, int anchor_x, int anchor_y, int normalize, int border);
 B200CV_API int b200cv_host_integral(const b200cvMat* src, const b200cvMat* sum, const b200cvMat* sqsum);
 B200CV_API int b200cv_host_resize(const b200cvMat* src, const b200cvMat* dst, int interpolation);

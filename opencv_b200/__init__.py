@@ -3,7 +3,7 @@
 The functions mirror the cv2 / cv:: names and argument meaning of the reference
 (modules/imgproc/include/opencv2/imgproc.hpp) for the calls on the hot path:
 
-    GaussianBlur, sepFilter2D, filter2D, Sobel, resize, warpAffine, warpPerspective, cvtColor,
+    GaussianBlur, sepFilter2D, filter2D, Sobel, Laplacian, resize, warpAffine, warpPerspective, cvtColor,
     matchTemplate, cornerHarris, cornerMinEigenVal, goodFeaturesToTrack, Canny, distanceTransform, sift_pyramid
 
 Inputs are torch CUDA tensors laid out like a cv::Mat -- (H, W) or (H, W, C), or a batch
@@ -262,6 +262,19 @@ def Sobel(src, ddepth, dx, dy, ksize=3, scale=1.0, delta=0.0, borderType=BORDER_
     ms, md = _pair(src, dst)
     _check(lib().b200cv_sobel(ctypes.byref(ms), ctypes.byref(md), int(dx), int(dy), int(ksize), ctypes.c_double(scale),
                               ctypes.c_double(delta), int(borderType), _stream_ptr(stream)), "Sobel")
+    return dst
+
+
+def Laplacian(src, ddepth, ksize=1, scale=1, delta=0, borderType=BORDER_DEFAULT, dst=None, stream=None):
+    """cv::Laplacian (imgproc.hpp): 8U -> 8U / 16S / 32F and 32F -> 32F, 1 to 4 channels, odd ksize 1..31; ddepth -1 keeps the source
+    depth.  A 64F destination (the cv2.Laplacian(gray, cv2.CV_64F) focus-measure idiom) is not offered."""
+    if not _is_torch(src):
+        from . import hal
+        return hal.Laplacian(src, ddepth, ksize, scale, delta, borderType, dst)
+    dst = dst if dst is not None else _new(src, dtype=_ddepth_dtype(src, ddepth))
+    ms, md = _pair(src, dst)
+    _check(lib().b200cv_laplacian(ctypes.byref(ms), ctypes.byref(md), int(ksize), ctypes.c_double(scale), ctypes.c_double(delta),
+                                  int(borderType), _stream_ptr(stream)), "Laplacian")
     return dst
 
 

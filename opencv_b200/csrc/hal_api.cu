@@ -177,6 +177,8 @@ extern "C" int b200cv_host_filter2d(const b200cvMat* s, const b200cvMat* d, cons
 { return host_pipeline(s, d, [=](const b200cvMat* a, const b200cvMat* b, void* st) { return b200cv_filter2d(a, b, k, kw, kh, ax, ay, delta, border, st); }); }
 extern "C" int b200cv_host_sobel(const b200cvMat* s, const b200cvMat* d, int dx, int dy, int ksize, double scale, double delta, int border)
 { return host_pipeline(s, d, [=](const b200cvMat* a, const b200cvMat* b, void* st) { return b200cv_sobel(a, b, dx, dy, ksize, scale, delta, border, st); }); }
+extern "C" int b200cv_host_laplacian(const b200cvMat* s, const b200cvMat* d, int ksize, double scale, double delta, int border)
+{ return host_pipeline(s, d, [=](const b200cvMat* a, const b200cvMat* b, void* st) { return b200cv_laplacian(a, b, ksize, scale, delta, border, st); }); }
 extern "C" int b200cv_host_box_filter(const b200cvMat* s, const b200cvMat* d, int kw, int kh, int ax, int ay, int normalize, int border)
 { return host_pipeline(s, d, [=](const b200cvMat* a, const b200cvMat* b, void* st) { return b200cv_box_filter(a, b, kw, kh, ax, ay, normalize, border, st); }); }
 extern "C" int b200cv_host_resize(const b200cvMat* s, const b200cvMat* d, int interp)

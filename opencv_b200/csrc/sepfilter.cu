@@ -590,7 +590,7 @@ int copy_impl(const b200cvMat* src, const b200cvMat* dst, void* stream)
 // Sobel taps (reference behaviour: getSobelKernels, modules/imgproc/src/deriv.cpp:96-160): the order-d derivative
 // kernel of size n is the binomial smoother (1+z)^(n-d-1) times the difference operator (z-1)^d, as polynomial
 // coefficients in z; built here by repeated 2-tap polynomial multiplication.
-static void sobel_kernel_1d(int ksize, int order, std::vector<float>& out)
+void sobel_kernel_1d(int ksize, int order, std::vector<float>& out)
 {
     std::vector<long long> poly(1, 1);
     auto mul2 = [&](long long c0, long long c1) {     // poly *= (c0 + c1*z)

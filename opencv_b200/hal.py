@@ -104,6 +104,14 @@ def Sobel(src, ddepth, dx, dy, ksize=3, scale=1.0, delta=0.0, borderType=BORDER_
     return dst
 
 
+def Laplacian(src, ddepth, ksize=1, scale=1.0, delta=0.0, borderType=BORDER_DEFAULT, dst=None):
+    dst = dst if dst is not None else _new(src, dtype=_ddt(src, ddepth))
+    ms, md = describe(src), describe(dst)
+    _check(lib().b200cv_host_laplacian(ctypes.byref(ms), ctypes.byref(md), int(ksize), ctypes.c_double(scale), ctypes.c_double(delta),
+                                       int(borderType)), "Laplacian")
+    return dst
+
+
 def distanceTransform(src, distanceType, maskSize, dst=None, dstType=CV_32F):
     """cv::distanceTransform over host 8UC1 arrays (b200cv_host_distance_transform): 8UC1 for DIST_L1 with dstType CV_8U, 32FC1
     otherwise; dst=src runs the 8-bit L1 call in place."""

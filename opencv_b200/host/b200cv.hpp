@@ -6,7 +6,7 @@
 //                                               (createGaussianFilter(type, type, ksize, sigma) -> apply(src, dst, stream))
 //   b200cv::GaussianBlur, sepFilter2D, filter2D, Sobel, resize, warpAffine, warpPerspective, cvtColor, matchTemplate, cornerHarris,
 //   cornerMinEigenVal, goodFeaturesToTrack,     same argument order and meaning as imgproc.hpp:1544,1723,1702,1862,2422,2450,2482,3736,
-//   Canny, distanceTransform                    3916,1948,1921,2096,1889,1907 and cv::distanceTransform, with a trailing Stream& like
+//   Canny, distanceTransform, Laplacian         3916,1948,1921,2096,1889,1907, cv::distanceTransform and cv::Laplacian, with a trailing Stream& like
 //                                               the cv::cuda:: functions
 // With -DB200CV_WITH_OPENCV (OpenCV headers on the include path) b200cv_opencv.hpp adds namespace b200cv::cuda: the same operations over
 // cv::InputArray / cv::OutputArray (cv::Mat, cv::cuda::GpuMat, cv::cuda::HostMem) with cv::cuda's Filter / Stream& shapes.
@@ -134,6 +134,11 @@ inline void Sobel(const GpuMat& src, GpuMat& dst, int ddepth, int dx, int dy, in
                   Stream& s = Stream::Null())
 { B200CV_DST(dst, src, makeType(ddepth < 0 ? B200CV_DEPTH(src.type()) : ddepth, src.channels())); b200cvMat a = src.desc(), b = dst.desc();
   check(b200cv_sobel(&a, &b, dx, dy, ksize, scale, delta, borderType, s.cudaPtr()), "Sobel"); }
+// cv::Laplacian: 8U -> 8U / 16S / 32F and 32F -> 32F, odd ksize 1..31
+inline void Laplacian(const GpuMat& src, GpuMat& dst, int ddepth, int ksize = 1, double scale = 1, double delta = 0, int borderType = BORDER_DEFAULT,
+                      Stream& s = Stream::Null())
+{ B200CV_DST(dst, src, makeType(ddepth < 0 ? B200CV_DEPTH(src.type()) : ddepth, src.channels())); b200cvMat a = src.desc(), b = dst.desc();
+  check(b200cv_laplacian(&a, &b, ksize, scale, delta, borderType, s.cudaPtr()), "Laplacian"); }
 // cv::integral (8UC1 -> 32SC1 sum of (rows+1) x (cols+1); optional 64FC1 sum of squares) and cv::cvtColorTwoPlane (NV12 / NV21, separate planes)
 inline void integral(const GpuMat& src, GpuMat& sum, Stream& s = Stream::Null())
 { sum.create(src.rows + 1, src.cols + 1, makeType(B200CV_32S, 1), src.frames); b200cvMat a = src.desc(), b = sum.desc();

@@ -214,6 +214,14 @@ inline void Sobel(cv::InputArray src, cv::OutputArray dst, int ddepth, int dx, i
     Arr a = input(src, "Sobel"), b = output(dst, a.m.rows, a.m.cols, dstType(ddepth, a.m.type), a.device, "Sobel");
     check(a.device ? b200cv_sobel(&a.m, &b.m, dx, dy, ksize, scale, delta, borderType, s.cudaPtr()) : b200cv_host_sobel(&a.m, &b.m, dx, dy, ksize, scale, delta, borderType), "Sobel");
 }
+// cv::Laplacian: a stock OpenCV built with the HAL already sends ksize 1 / 3 here through filter2D; ksize 5..31 only through this call
+inline void Laplacian(cv::InputArray src, cv::OutputArray dst, int ddepth, int ksize = 1, double scale = 1, double delta = 0, int borderType = cv::BORDER_DEFAULT,
+                      Stream& s = Stream::Null())
+{
+    Arr a = input(src, "Laplacian"), b = output(dst, a.m.rows, a.m.cols, dstType(ddepth, a.m.type), a.device, "Laplacian");
+    check(a.device ? b200cv_laplacian(&a.m, &b.m, ksize, scale, delta, borderType, s.cudaPtr()) : b200cv_host_laplacian(&a.m, &b.m, ksize, scale, delta, borderType),
+          "Laplacian");
+}
 inline void resize(cv::InputArray src, cv::OutputArray dst, cv::Size dsize, double fx = 0, double fy = 0, int interpolation = cv::INTER_LINEAR, Stream& s = Stream::Null())
 {
     Arr a = input(src, "resize");
