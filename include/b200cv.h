@@ -105,6 +105,19 @@ extern "C" {
 #define B200CV_DIST_MASK_3 3
 #define B200CV_DIST_MASK_5 5
 
+/* cv::MorphTypes and cv::MorphShapes (imgproc.hpp) */
+#define B200CV_MORPH_ERODE 0
+#define B200CV_MORPH_DILATE 1
+#define B200CV_MORPH_OPEN 2
+#define B200CV_MORPH_CLOSE 3
+#define B200CV_MORPH_GRADIENT 4
+#define B200CV_MORPH_TOPHAT 5
+#define B200CV_MORPH_BLACKHAT 6
+#define B200CV_MORPH_HITMISS 7
+#define B200CV_MORPH_RECT 0
+#define B200CV_MORPH_CROSS 1
+#define B200CV_MORPH_ELLIPSE 2
+
 /* A (batch of) device image(s).  frames<=1 means a single frame (frame_step ignored). */
 typedef struct b200cvMat {
     void*  data;        /* device pointer to pixel (0,0) of frame 0 */
@@ -181,6 +194,26 @@ B200CV_API int b200cv_sobel(const b200cvMat* src, const b200cvMat* dst, int dx, 
  * B200CV_ERR_BAD_ARG.  Borders CONSTANT (zero), REPLICATE, REFLECT, REFLECT_101, each with or without ISOLATED (a view has no parent,
  * so ISOLATED changes nothing); WRAP returns B200CV_NOT_IMPLEMENTED.  src == dst is refused.  Batches: one launch for all frames. */
 B200CV_API int b200cv_laplacian(const b200cvMat* src, const b200cvMat* dst, int ksize, double scale, double delta, int border, void* stream);
+/* replaces cv::erode / cv::dilate (op B200CV_MORPH_ERODE / DILATE) and cv::morphologyEx (ops ERODE..BLACKHAT) (imgproc.hpp;
+ * morph.dispatch.cpp), bit-exact.  8U, 16U, 16S and 32F, 1 to 4 channels; dst has the type and size of src.  The element is a host byte
+ * mask of kh rows of kw bytes, kernel_step apart, non-zero meaning "in the element"; kernel_data NULL or kw / kh 0 is the empty element,
+ * which is cv::erode / cv::dilate's (1+2*iterations)^2 rectangle for ops 0 and 1 and morphologyEx's 3x3 rectangle for ops 2 to 6
+ * (morphologyEx with op 0 or 1 and no element passes the 3x3 rectangle itself).  Anchor (-1, -1) is the centre.  iterations == 0 or a
+ * 1x1 element copies; an all-ones element with iterations > 1 grows as the reference grows it and runs once; any other element runs
+ * max(iterations, 1) passes.  border_value: NULL, or four DBL_MAX, is the reference's default (the depth's maximum for erode, its minimum
+ * for dilate; +-FLT_MAX for 32F); otherwise saturate_cast per channel.  Borders CONSTANT, REPLICATE, REFLECT, REFLECT_101, with or
+ * without ISOLATED.  Batches: one launch sequence per call.  32F windows holding a NaN, or both -0.0 and +0.0, may pick another operand
+ * than the reference does (whose choice depends on the column).
+ * A rectangle's reach past a line's ends is cut to twice the line's length, which changes no value (so 3x3 with 2^29 iterations runs
+ * in time bounded by the image).
+ * MORPH_HITMISS, 64F and other depths, BORDER_WRAP, a non-rectangular element larger than 63x63, a rectangle over 32 on a line so long
+ * that len + 2 * (its cut size) exceeds INT_MAX: B200CV_NOT_IMPLEMENTED.  An anchor
+ * outside the element, an empty element with iterations < 0 in ops 0 / 1, an element larger than 1x1 without a non-zero entry, a dst of
+ * another type or size, src and dst overlapping, W * H >= 2^31, (W + 190) * cn >= 2^31 (a row of elements and its widest apron):
+ * B200CV_ERR_BAD_ARG.  Refusals leave dst untouched. */
+B200CV_API int b200cv_morphology(const b200cvMat* src, const b200cvMat* dst, int op, const unsigned char* kernel_data, size_t kernel_step,
+                                 int kw, int kh, int anchor_x, int anchor_y, int iterations, int border, const double border_value[4],
+                                 void* stream);
 /* replaces cv::boxFilter / cv::blur (imgproc.hpp:1603, :1659; box_filter.dispatch.cpp:440-498).  dst depth picks ddepth:
  * 8U->8U, 8U->32F, 32F->32F; anchor (-1,-1) = centre; borders CONSTANT (zeros), REPLICATE, REFLECT, REFLECT_101; ksize <= 128x128. */
 B200CV_API int b200cv_box_filter(const b200cvMat* src, const b200cvMat* dst, int ksize_w, int ksize_h, int anchor_x, int anchor_y,

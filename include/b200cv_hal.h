@@ -133,6 +133,10 @@ B200CV_API int b200cv_host_filter2d(const b200cvMat* src, const b200cvMat* dst, 
                                     double delta, int border);
 B200CV_API int b200cv_host_sobel(const b200cvMat* src, const b200cvMat* dst, int dx, int dy, int ksize, double scale, double delta, int border);
 B200CV_API int b200cv_host_laplacian(const b200cvMat* src, const b200cvMat* dst, int ksize, double scale, double delta, int border);
+/* cv::erode / cv::dilate / cv::morphologyEx over host frames; arguments as b200cv_morphology takes them.  No cv_hal_morph hook is
+ * registered (see INTEGRATION.md), so there is no hal_ni_* counterpart. */
+B200CV_API int b200cv_host_morphology(const b200cvMat* src, const b200cvMat* dst, int op, const unsigned char* kernel_data, size_t kernel_step,
+                                      int kw, int kh, int anchor_x, int anchor_y, int iterations, int border, const double border_value[4]);
 B200CV_API int b200cv_host_box_filter(const b200cvMat* src, const b200cvMat* dst, int ksize_w, int ksize_h, int anchor_x, int anchor_y, int normalize, int border);
 B200CV_API int b200cv_host_integral(const b200cvMat* src, const b200cvMat* sum, const b200cvMat* sqsum);
 B200CV_API int b200cv_host_resize(const b200cvMat* src, const b200cvMat* dst, int interpolation);

@@ -3,7 +3,7 @@
 The functions mirror the cv2 / cv:: names and argument meaning of the reference
 (modules/imgproc/include/opencv2/imgproc.hpp) for the calls on the hot path:
 
-    GaussianBlur, sepFilter2D, filter2D, Sobel, Laplacian, resize, warpAffine, warpPerspective, cvtColor,
+    GaussianBlur, sepFilter2D, filter2D, Sobel, Laplacian, erode, dilate, morphologyEx, resize, warpAffine, warpPerspective, cvtColor,
     matchTemplate, cornerHarris, cornerMinEigenVal, goodFeaturesToTrack, Canny, distanceTransform, sift_pyramid
 
 Inputs are torch CUDA tensors laid out like a cv::Mat -- (H, W) or (H, W, C), or a batch
@@ -34,6 +34,9 @@ TM_SQDIFF, TM_SQDIFF_NORMED, TM_CCORR, TM_CCORR_NORMED, TM_CCOEFF, TM_CCOEFF_NOR
 # cv::DistanceTypes and cv::DistanceTransformMasks
 DIST_USER, DIST_L1, DIST_L2, DIST_C, DIST_L12, DIST_FAIR, DIST_WELSCH, DIST_HUBER = -1, 1, 2, 3, 4, 5, 6, 7
 DIST_MASK_3, DIST_MASK_5, DIST_MASK_PRECISE = 3, 5, 0
+# cv::MorphTypes and cv::MorphShapes
+MORPH_ERODE, MORPH_DILATE, MORPH_OPEN, MORPH_CLOSE, MORPH_GRADIENT, MORPH_TOPHAT, MORPH_BLACKHAT, MORPH_HITMISS = range(8)
+MORPH_RECT, MORPH_CROSS, MORPH_ELLIPSE = 0, 1, 2
 COLOR_BGR2BGRA, COLOR_BGRA2BGR, COLOR_BGR2RGBA, COLOR_RGBA2BGR, COLOR_BGR2RGB, COLOR_BGRA2RGBA = range(6)
 COLOR_RGB2BGRA, COLOR_BGRA2RGB, COLOR_RGB2BGR, COLOR_RGBA2BGRA = COLOR_BGR2RGBA, COLOR_RGBA2BGR, COLOR_BGR2RGB, COLOR_BGRA2RGBA
 COLOR_BGR2GRAY, COLOR_RGB2GRAY, COLOR_GRAY2BGR, COLOR_GRAY2BGRA, COLOR_BGRA2GRAY, COLOR_RGBA2GRAY = 6, 7, 8, 9, 10, 11
@@ -275,6 +278,91 @@ def Laplacian(src, ddepth, ksize=1, scale=1, delta=0, borderType=BORDER_DEFAULT,
     ms, md = _pair(src, dst)
     _check(lib().b200cv_laplacian(ctypes.byref(ms), ctypes.byref(md), int(ksize), ctypes.c_double(scale), ctypes.c_double(delta),
                                   int(borderType), _stream_ptr(stream)), "Laplacian")
+    return dst
+
+
+def getStructuringElement(shape, ksize, anchor=(-1, -1)):
+    """cv::getStructuringElement (morph.dispatch.cpp), computed on the host: a (h, w) uint8 array of 0 / 1 for MORPH_RECT, MORPH_CROSS
+    or MORPH_ELLIPSE; a 1x1 size is always a rectangle.  Ellipse rows span c +- round(c * sqrt((r^2 - dy^2) / r^2)), half to even."""
+    import math
+    import numpy as np
+    w, h = int(ksize[0]), int(ksize[1])
+    if shape not in (MORPH_RECT, MORPH_CROSS, MORPH_ELLIPSE):
+        raise B200cvError("getStructuringElement: unknown shape %r" % (shape,))
+    ax = w // 2 if anchor[0] == -1 else int(anchor[0])
+    ay = h // 2 if anchor[1] == -1 else int(anchor[1])
+    if not (0 <= ax < w and 0 <= ay < h):
+        raise B200cvError("getStructuringElement: the anchor must lie inside the element")
+    if (w, h) == (1, 1):
+        shape = MORPH_RECT
+    r, c = h // 2, w // 2
+    inv_r2 = 1.0 / (float(r) * r) if r else 0.0
+    elem = np.zeros((h, w), np.uint8)
+    for i in range(h):
+        j1 = j2 = 0
+        if shape == MORPH_RECT or (shape == MORPH_CROSS and i == ay):
+            j2 = w
+        elif shape == MORPH_CROSS:
+            j1, j2 = ax, ax + 1
+        elif abs(i - r) <= r:
+            dx = int(round(c * math.sqrt((r * r - (i - r) * (i - r)) * inv_r2)))
+            j1, j2 = max(c - dx, 0), min(c + dx + 1, w)
+        elem[i, j1:j2] = 1
+    return elem
+
+
+def _morph_args(kernel, borderValue, entry_ex):
+    """(k, kp, kw, kh, bv) for b200cv_morphology / b200cv_host_morphology: k is the element as a contiguous 0 / 1 byte mask (None for
+    the empty element: None or any array, list or tensor of size 0) and kp its pointer, kw / kh its size, bv the double[4] border value
+    (None: the reference's default, four DBL_MAX).  entry_ex (morphologyEx) turns the empty element into the 3x3 rectangle for every op,
+    as the reference's morphologyEx does; erode / dilate keep it empty, their own (1 + 2 * iterations)^2 rule."""
+    import numpy as np
+    if kernel is not None and _is_torch(kernel):
+        kernel = kernel.cpu().numpy()
+    if (kernel is None or np.asarray(kernel).size == 0) and entry_ex:
+        kernel = np.ones((3, 3), np.uint8)
+    if kernel is None or np.asarray(kernel).size == 0:
+        k, kw, kh = None, 0, 0
+    else:
+        k = np.ascontiguousarray(np.asarray(kernel) != 0, dtype=np.uint8)
+        if k.ndim == 1:
+            k = k.reshape(1, -1)
+        kh, kw = k.shape
+    if borderValue is None:
+        bv = [1.7976931348623157e308] * 4
+    else:
+        vals = [float(v) for v in (borderValue if hasattr(borderValue, "__len__") else (borderValue,))]
+        bv = (vals + [0.0] * 4)[:4]
+    kp = None if k is None else k.ctypes.data_as(ctypes.POINTER(ctypes.c_ubyte))
+    return k, kp, kw, kh, (ctypes.c_double * 4)(*bv)
+
+
+def morphologyEx(src, op, kernel, dst=None, anchor=(-1, -1), iterations=1, borderType=BORDER_CONSTANT, borderValue=None, stream=None):
+    """cv::morphologyEx (imgproc.hpp): MORPH_ERODE .. MORPH_BLACKHAT over 8U / 16U / 16S / 32F images of 1 to 4 channels, or (N, H, W, C)
+    batches.  kernel: any 2-D array, non-zero meaning "in the element"; None or an empty array, list or tensor is the 3x3 rectangle.  borderValue None is the
+    reference's morphologyDefaultBorderValue().  MORPH_HITMISS is not offered."""
+    return _morphology(src, op, kernel, dst, anchor, iterations, borderType, borderValue, stream, True)
+
+
+def erode(src, kernel, dst=None, anchor=(-1, -1), iterations=1, borderType=BORDER_CONSTANT, borderValue=None, stream=None):
+    """cv::erode (imgproc.hpp); kernel None is the reference's empty element, a (1+2*iterations)^2 rectangle applied once"""
+    return _morphology(src, MORPH_ERODE, kernel, dst, anchor, iterations, borderType, borderValue, stream)
+
+
+def dilate(src, kernel, dst=None, anchor=(-1, -1), iterations=1, borderType=BORDER_CONSTANT, borderValue=None, stream=None):
+    """cv::dilate (imgproc.hpp); kernel None is the reference's empty element, a (1+2*iterations)^2 rectangle applied once"""
+    return _morphology(src, MORPH_DILATE, kernel, dst, anchor, iterations, borderType, borderValue, stream)
+
+
+def _morphology(src, op, kernel, dst, anchor, iterations, borderType, borderValue, stream, entry_ex=False):
+    if not _is_torch(src):
+        from . import hal
+        return hal._morphology(src, op, kernel, dst, anchor, iterations, borderType, borderValue, entry_ex)
+    dst = dst if dst is not None else _new(src)
+    ms, md = _pair(src, dst)
+    k, kp, kw, kh, bv = _morph_args(kernel, borderValue, entry_ex)
+    _check(lib().b200cv_morphology(ctypes.byref(ms), ctypes.byref(md), int(op), kp, ctypes.c_size_t(kw), int(kw), int(kh), int(anchor[0]),
+                                   int(anchor[1]), int(iterations), int(borderType), bv, _stream_ptr(stream)), "morphology")
     return dst
 
 

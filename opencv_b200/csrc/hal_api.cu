@@ -200,6 +200,10 @@ extern "C" int b200cv_host_corner_min_eigen_val(const b200cvMat* s, const b200cv
 { return host_pipeline(s, d, [=](const b200cvMat* a, const b200cvMat* b, void* st) { return b200cv_corner_min_eigen_val(a, b, bs, ks, border, st); }); }
 extern "C" int b200cv_host_canny(const b200cvMat* s, const b200cvMat* d, double t1, double t2, int aperture, int l2)
 { return host_pipeline(s, d, [=](const b200cvMat* a, const b200cvMat* b, void* st) { return b200cv_canny(a, b, t1, t2, aperture, l2, st); }); }
+extern "C" int b200cv_host_morphology(const b200cvMat* s, const b200cvMat* d, int op, const unsigned char* kernel_data, size_t kernel_step, int kw,
+                                      int kh, int anchor_x, int anchor_y, int iterations, int border, const double border_value[4])
+{ return host_pipeline(s, d, [=](const b200cvMat* a, const b200cvMat* b, void* st) {
+      return b200cv_morphology(a, b, op, kernel_data, kernel_step, kw, kh, anchor_x, anchor_y, iterations, border, border_value, st); }); }
 extern "C" int b200cv_host_distance_transform(const b200cvMat* s, const b200cvMat* d, int distance_type, int mask_size)
 { return host_pipeline(s, d, [=](const b200cvMat* a, const b200cvMat* b, void* st) { return b200cv_distance_transform(a, b, distance_type, mask_size, st); }); }
 

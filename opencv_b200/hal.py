@@ -112,6 +112,31 @@ def Laplacian(src, ddepth, ksize=1, scale=1.0, delta=0.0, borderType=BORDER_DEFA
     return dst
 
 
+def _morphology(src, op, kernel, dst, anchor, iterations, borderType, borderValue, entry_ex=False):
+    from . import _morph_args
+    dst = dst if dst is not None else _new(src)
+    ms, md = describe(src), describe(dst)
+    k, kp, kw, kh, bv = _morph_args(kernel, borderValue, entry_ex)
+    _check(lib().b200cv_host_morphology(ctypes.byref(ms), ctypes.byref(md), int(op), kp, ctypes.c_size_t(kw), int(kw), int(kh),
+                                        int(anchor[0]), int(anchor[1]), int(iterations), int(borderType), bv), "morphology")
+    return dst
+
+
+def erode(src, kernel, dst=None, anchor=(-1, -1), iterations=1, borderType=BORDER_CONSTANT, borderValue=None):
+    """cv::erode over host arrays (b200cv_host_morphology)"""
+    return _morphology(src, 0, kernel, dst, anchor, iterations, borderType, borderValue)
+
+
+def dilate(src, kernel, dst=None, anchor=(-1, -1), iterations=1, borderType=BORDER_CONSTANT, borderValue=None):
+    """cv::dilate over host arrays (b200cv_host_morphology)"""
+    return _morphology(src, 1, kernel, dst, anchor, iterations, borderType, borderValue)
+
+
+def morphologyEx(src, op, kernel, dst=None, anchor=(-1, -1), iterations=1, borderType=BORDER_CONSTANT, borderValue=None):
+    """cv::morphologyEx over host arrays (b200cv_host_morphology); kernel None or empty is the 3x3 rectangle"""
+    return _morphology(src, op, kernel, dst, anchor, iterations, borderType, borderValue, True)
+
+
 def distanceTransform(src, distanceType, maskSize, dst=None, dstType=CV_32F):
     """cv::distanceTransform over host 8UC1 arrays (b200cv_host_distance_transform): 8UC1 for DIST_L1 with dstType CV_8U, 32FC1
     otherwise; dst=src runs the 8-bit L1 call in place."""

@@ -6,8 +6,9 @@
 //                                               (createGaussianFilter(type, type, ksize, sigma) -> apply(src, dst, stream))
 //   b200cv::GaussianBlur, sepFilter2D, filter2D, Sobel, resize, warpAffine, warpPerspective, cvtColor, matchTemplate, cornerHarris,
 //   cornerMinEigenVal, goodFeaturesToTrack,     same argument order and meaning as imgproc.hpp:1544,1723,1702,1862,2422,2450,2482,3736,
-//   Canny, distanceTransform, Laplacian         3916,1948,1921,2096,1889,1907, cv::distanceTransform and cv::Laplacian, with a trailing Stream& like
-//                                               the cv::cuda:: functions
+//   Canny, distanceTransform, Laplacian,        3916,1948,1921,2096,1889,1907, cv::distanceTransform, cv::Laplacian and cv::erode / dilate /
+//   erode, dilate, morphologyEx                 morphologyEx (the element as a byte mask and its Size), with a trailing Stream& like the
+//                                               cv::cuda:: functions
 // With -DB200CV_WITH_OPENCV (OpenCV headers on the include path) b200cv_opencv.hpp adds namespace b200cv::cuda: the same operations over
 // cv::InputArray / cv::OutputArray (cv::Mat, cv::cuda::GpuMat, cv::cuda::HostMem) with cv::cuda's Filter / Stream& shapes.
 // Errors: the C ABI status is turned into b200cv::Error (std::runtime_error); NOT_IMPLEMENTED is b200cv::NotImplemented.
@@ -15,6 +16,7 @@
 #ifdef B200CV_WITH_OPENCV
 #include <opencv2/core.hpp>
 #endif
+#include <cfloat>
 #include <memory>
 #include <stdexcept>
 #include <string>
@@ -139,6 +141,28 @@ inline void Laplacian(const GpuMat& src, GpuMat& dst, int ddepth, int ksize = 1,
                       Stream& s = Stream::Null())
 { B200CV_DST(dst, src, makeType(ddepth < 0 ? B200CV_DEPTH(src.type()) : ddepth, src.channels())); b200cvMat a = src.desc(), b = dst.desc();
   check(b200cv_laplacian(&a, &b, ksize, scale, delta, borderType, s.cudaPtr()), "Laplacian"); }
+// cv::erode / cv::dilate / cv::morphologyEx: 8U / 16U / 16S / 32F, 1 to 4 channels.  The element is a host byte mask of ksize.height rows
+// of ksize.width bytes (non-zero = in the element); nullptr is the empty element (erode / dilate: a (1+2*iterations)^2 rectangle;
+// morphologyEx: 3x3).  The default borderValue is morphologyDefaultBorderValue() (four DBL_MAX).
+inline Scalar morphologyDefaultBorderValue() { return Scalar(DBL_MAX, DBL_MAX, DBL_MAX, DBL_MAX); }
+inline void morphologyEx(const GpuMat& src, GpuMat& dst, int op, const unsigned char* kernel, Size ksize, Point anchor = Point(-1, -1),
+                         int iterations = 1, int borderType = BORDER_CONSTANT, const Scalar& borderValue = morphologyDefaultBorderValue(),
+                         Stream& s = Stream::Null())
+{ static const unsigned char k3[9] = {1, 1, 1, 1, 1, 1, 1, 1, 1};
+  if (!kernel || ksize.width <= 0 || ksize.height <= 0) { kernel = k3; ksize = Size(3, 3); }
+  B200CV_DST(dst, src, src.type()); b200cvMat a = src.desc(), b = dst.desc();
+  check(b200cv_morphology(&a, &b, op, kernel, (size_t)ksize.width, ksize.width, ksize.height, anchor.x, anchor.y, iterations, borderType,
+                          borderValue.val, s.cudaPtr()), "morphologyEx"); }
+inline void erode(const GpuMat& src, GpuMat& dst, const unsigned char* kernel, Size ksize, Point anchor = Point(-1, -1), int iterations = 1,
+                  int borderType = BORDER_CONSTANT, const Scalar& borderValue = morphologyDefaultBorderValue(), Stream& s = Stream::Null())
+{ B200CV_DST(dst, src, src.type()); b200cvMat a = src.desc(), b = dst.desc();
+  check(b200cv_morphology(&a, &b, B200CV_MORPH_ERODE, kernel, (size_t)ksize.width, ksize.width, ksize.height, anchor.x, anchor.y, iterations,
+                          borderType, borderValue.val, s.cudaPtr()), "erode"); }
+inline void dilate(const GpuMat& src, GpuMat& dst, const unsigned char* kernel, Size ksize, Point anchor = Point(-1, -1), int iterations = 1,
+                   int borderType = BORDER_CONSTANT, const Scalar& borderValue = morphologyDefaultBorderValue(), Stream& s = Stream::Null())
+{ B200CV_DST(dst, src, src.type()); b200cvMat a = src.desc(), b = dst.desc();
+  check(b200cv_morphology(&a, &b, B200CV_MORPH_DILATE, kernel, (size_t)ksize.width, ksize.width, ksize.height, anchor.x, anchor.y, iterations,
+                          borderType, borderValue.val, s.cudaPtr()), "dilate"); }
 // cv::integral (8UC1 -> 32SC1 sum of (rows+1) x (cols+1); optional 64FC1 sum of squares) and cv::cvtColorTwoPlane (NV12 / NV21, separate planes)
 inline void integral(const GpuMat& src, GpuMat& sum, Stream& s = Stream::Null())
 { sum.create(src.rows + 1, src.cols + 1, makeType(B200CV_32S, 1), src.frames); b200cvMat a = src.desc(), b = sum.desc();

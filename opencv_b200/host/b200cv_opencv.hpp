@@ -222,6 +222,33 @@ inline void Laplacian(cv::InputArray src, cv::OutputArray dst, int ddepth, int k
     check(a.device ? b200cv_laplacian(&a.m, &b.m, ksize, scale, delta, borderType, s.cudaPtr()) : b200cv_host_laplacian(&a.m, &b.m, ksize, scale, delta, borderType),
           "Laplacian");
 }
+// cv::erode / cv::dilate / cv::morphologyEx (MORPH_ERODE .. MORPH_BLACKHAT): no cv_hal_morph hook is registered (INTEGRATION.md), so a
+// stock OpenCV keeps its own morphology; call these instead.  kernel: any 8-bit single-channel mask, or empty.
+inline void morphology_(int op, cv::InputArray src, cv::OutputArray dst, cv::InputArray kernel, cv::Point anchor, int iterations, int borderType,
+                        const cv::Scalar& borderValue, Stream& s, const char* what)
+{
+    Arr a = input(src, what), b = output(dst, a.m.rows, a.m.cols, a.m.type, a.device, what);
+    cv::Mat k = kernel.getMat();
+    if (!k.empty()) { CV_Assert(k.type() == CV_8UC1); k = k.isContinuous() ? k : k.clone(); }
+    const unsigned char* kp = k.empty() ? nullptr : k.ptr();
+    const size_t kstep = k.empty() ? 0 : k.step[0];
+    check(a.device ? b200cv_morphology(&a.m, &b.m, op, kp, kstep, k.cols, k.rows, anchor.x, anchor.y, iterations, borderType, borderValue.val, s.cudaPtr())
+                   : b200cv_host_morphology(&a.m, &b.m, op, kp, kstep, k.cols, k.rows, anchor.x, anchor.y, iterations, borderType, borderValue.val),
+          what);
+}
+inline void erode(cv::InputArray src, cv::OutputArray dst, cv::InputArray kernel, cv::Point anchor = cv::Point(-1, -1), int iterations = 1,
+                  int borderType = cv::BORDER_CONSTANT, const cv::Scalar& borderValue = cv::morphologyDefaultBorderValue(), Stream& s = Stream::Null())
+{ morphology_(cv::MORPH_ERODE, src, dst, kernel, anchor, iterations, borderType, borderValue, s, "erode"); }
+inline void dilate(cv::InputArray src, cv::OutputArray dst, cv::InputArray kernel, cv::Point anchor = cv::Point(-1, -1), int iterations = 1,
+                   int borderType = cv::BORDER_CONSTANT, const cv::Scalar& borderValue = cv::morphologyDefaultBorderValue(), Stream& s = Stream::Null())
+{ morphology_(cv::MORPH_DILATE, src, dst, kernel, anchor, iterations, borderType, borderValue, s, "dilate"); }
+inline void morphologyEx(cv::InputArray src, cv::OutputArray dst, int op, cv::InputArray kernel, cv::Point anchor = cv::Point(-1, -1), int iterations = 1,
+                         int borderType = cv::BORDER_CONSTANT, const cv::Scalar& borderValue = cv::morphologyDefaultBorderValue(), Stream& s = Stream::Null())
+{
+    cv::Mat k = kernel.getMat();
+    if (k.empty()) k = cv::getStructuringElement(cv::MORPH_RECT, cv::Size(3, 3));
+    morphology_(op, src, dst, k, anchor, iterations, borderType, borderValue, s, "morphologyEx");
+}
 inline void resize(cv::InputArray src, cv::OutputArray dst, cv::Size dsize, double fx = 0, double fy = 0, int interpolation = cv::INTER_LINEAR, Stream& s = Stream::Null())
 {
     Arr a = input(src, "resize");
